@@ -21,7 +21,7 @@ Own arm
              tower, C4 LightGCN L=3, C5 shape on one GPU (and row-sharded when N > 1), rank / full_rank / KPIs / sampling /
              epoch permutation, and one step-time line each for FM, NFM, NGCF (SURVEY 8(f) ranks 3-4).
   parity_check (N > 1)  3 global steps on a 48 K-triple slice: sharded run vs the single-GPU kernel on the same batches.
-  cpu_baseline  the REAL reference (oracle/_ref = /root/reference installed unmodified, oracle/build_ref.py) running
+  cpu_baseline  the REAL reference (oracle/_ref: the daisyRec package installed unmodified by oracle/build_ref.py) running
              daisy.model.MFRecommender.MF.fit over its own DataLoader on this host's cores, bounded sample, in a
              subprocess with the GPUs hidden.
 Reference arm (--impl reference): the same real-reference run for K steps after W warm-up steps (rank 0 only).
@@ -52,7 +52,7 @@ def dist_env():
 
 
 class ClockSampler:
-    """nvidia-smi sampler running beside the timed region (B200_PROFILING.md clocks line)."""
+    """nvidia-smi sampler running beside the timed region: SM clock and throttle reasons of the measured GPU."""
     Q = ("index,clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.active,clocks_event_reasons.hw_slowdown,"
          "clocks_event_reasons.hw_thermal_slowdown,clocks_event_reasons.sw_thermal_slowdown,"
          "clocks_event_reasons.sw_power_cap")
@@ -110,20 +110,7 @@ def measured_peaks():
             return float(json.load(open(p))["hbm_gbs"]), "MEASURED_PEAKS.json hbm_gbs (measured copy bandwidth)"
         except Exception:  # noqa: BLE001
             pass
-    return 6650.0, "fallback 6.65 TB/s (B200_PROFILING.md)"
-
-
-def profiled_traffic(factors, batch):
-    """dram bytes per STEP from the committed ncu capture (profiles/traffic.json), else None."""
-    p = os.path.join(ROOT, "profiles", "traffic.json")
-    if os.path.exists(p):
-        try:
-            t = json.load(open(p))
-            if t.get("factors") == factors and t.get("batch") == batch:
-                return t.get("dram_bytes_per_step"), t.get("source", "profiles/traffic.json")
-        except Exception:  # noqa: BLE001
-            pass
-    return None, None
+    return 3350.0, "fallback 3.35 TB/s (H100 SXM data sheet, HBM3)"
 
 
 def build_workload(shape, device, num_ng, seed, sampler):
@@ -150,13 +137,37 @@ def workload_config(args, world):
     from daisyrec_b200.utils.synthetic import SHAPES
     U, I, nnz = SHAPES[args.shape]
     T = nnz * args.num_ng
+    tab_mb = (U + I) * args.factors * 4 / 1e6
     return {"workload": f"MF+BPR synthetic {args.shape} shape ({U}x{I}, nnz={nnz}, num_ng={args.num_ng} -> {T} "
                         f"triples/epoch), factors={args.factors}, SGD lr=0.01 reg=0.001/0.001",
             "batch_size": args.batch, "global_batch": args.batch * world, "factors": args.factors,
             "triples_per_epoch": T, "optimizer": "sgd",
             "parallelism": "single GPU" if world == 1 else f"user-row-sharded P x{world}, replicated Q",
-            "l2": "index planes (12 B/triple, all K steps) exceed L2 and are streamed once; the factor tables "
-                  "(42 MB at F=64) are persistent model state reused by every step and stay L2-resident by design"}
+            "l2": f"index planes (12 B/triple, all K steps) exceed L2 and are streamed once; the factor tables ({tab_mb:.0f} MB) "
+                  f"and their gradient accumulators (as much again) are reused by every step and "
+                  f"{'exceed' if 2 * tab_mb > 50 else 'fit'} the 50 MB L2 of an H100"}
+
+
+DUMP_BYTES = 64 << 20
+
+
+def dump_outputs(out_dir, arrays, seed=0):
+    """Write each array as out_dir/<name>.npy (float32 / float64).  Arrays above their share of the 64 MB budget are
+    replaced by a fixed seeded sample of their rows, so two builds run with the same arguments dump the same elements."""
+    os.makedirs(out_dir, exist_ok=True)
+    share = DUMP_BYTES // max(1, len(arrays))
+    for name, a in arrays.items():
+        a = np.ascontiguousarray(a)
+        assert a.dtype in (np.float32, np.float64), (name, a.dtype)
+        if a.nbytes > share:
+            rng = np.random.default_rng(seed)
+            row_bytes = a.nbytes // a.shape[0]
+            if share >= row_bytes:                 # whole rows
+                a = a[np.sort(rng.choice(a.shape[0], share // row_bytes, replace=False))]
+            else:                                  # one row alone exceeds the share: a sample of the elements
+                flat = a.reshape(-1)
+                a = flat[np.sort(rng.choice(flat.size, share // a.itemsize, replace=False))]
+        np.save(os.path.join(out_dir, name + ".npy"), a)
 
 
 def timed_ms(fn, warm, reps):
@@ -299,7 +310,7 @@ def run_reference(args):
 
 
 def run_reference_port(args, cfg, cores):
-    """oracle/_ref missing (the recipe never ran where /root/reference exists): time the pinned PyTorch-CPU port."""
+    """oracle/_ref missing (build() found no reference source tree): time the pinned PyTorch-CPU port."""
     from daisyrec_b200.utils.synthetic import SHAPES, init_tables
     from oracle.torch_port import TorchMFBaseline
     U, I, _ = SHAPES[args.shape]
@@ -380,7 +391,7 @@ def roof(achieved_gbs, kernel, alg_bytes, note=None):
 
 
 def cfg_c3_neumf(args, dev, d, planes):
-    """BASELINE config 3: NeuMF + BPR, ML-20M shape, F=32, tower 128->64->32, Adam, bf16 tcgen05 tower."""
+    """BASELINE config 3: NeuMF + BPR, ML-20M shape, F=32, tower 128->64->32, Adam, bf16 wgmma tower."""
     from daisyrec_b200 import ops
     U, I = d["user_num"], d["item_num"]
     F, L, B = 32, 2, args.batch
@@ -402,13 +413,13 @@ def cfg_c3_neumf(args, dev, d, planes):
         ms = timed_ms(fn, 3, 8 if td else 4)
         bpt = 3 * (F + D) * 4 * 2 + 12
         kern = {2: "neumf_fused_kernel (gather + tower fwd/bwd + head + scatter in one CTA per tile) + table sweeps",
-                1: "layer-wise tcgen05 GEMMs + head + table sweeps", 0: "layer-wise fp32 GEMMs + head + table sweeps"}[td]
+                1: "layer-wise wgmma GEMMs + head + table sweeps", 0: "layer-wise fp32 GEMMs + head + table sweeps"}[td]
         out[name] = {"value": B / ms * 1e3, "unit": UNIT, "ms_per_step": ms, "batch": B,
                      "roofline": roof(B * bpt / ms / 1e6, kern, bpt)}
         del ws
     res = out["fused"]
-    res["workload"] = (f"NeuMF+BPR synthetic ml-20m shape, factors={F}, num_layers={L} (tower {2*D}->{D}->{F}), Adam, bf16 tcgen05 "
-                       "tower fused per 64-triple tile (activations in shared / tensor memory)")
+    res["workload"] = (f"NeuMF+BPR synthetic ml-20m shape, factors={F}, num_layers={L} (tower {2*D}->{D}->{F}), Adam, bf16 wgmma "
+                       "tower fused per 64-triple tile (activations in shared memory, accumulators in registers)")
     res["layerwise_bf16_tower"] = out["bf16"]
     res["fp32_tower"] = out["fp32"]
     return res
@@ -443,7 +454,7 @@ def cfg_c4_lightgcn(args, dev):
         alg = 2 * L * (nnzA * (8 + 4 * F) + (U + I) * 4 * F) + B * (24 * F + 12)
         out[f"batch_{B}"] = {"value": B / ms * 1e3, "unit": UNIT, "ms_per_step": ms, "batch": B,
                              "roofline": roof(alg / ms / 1e6, "spmm_seg_kernel x 2L + BPR phases + Adam sweep (per step)", alg,
-                                              "upper-bound algorithmic bytes: neighbour-row gathers are mostly L2 hits")}
+                                              "upper-bound algorithmic bytes: neighbour-row gathers that hit L2 are counted too")}
         del ws
     out["value"], out["unit"], out["ms_per_step"] = out["batch_65536"]["value"], UNIT, out["batch_65536"]["ms_per_step"]
     return out
@@ -666,6 +677,8 @@ def run_own(args):
     torch.cuda.set_device(local)
     dev = torch.device("cuda", local)
     if world > 1:
+        if args.dump_outputs:
+            raise RuntimeError("--dump-outputs writes what the single-GPU own arm computed: run it without torchrun")
         import torch.distributed as dist
         dist.init_process_group("nccl", device_id=dev)
         return run_sharded(args, rank, local, world, dev)
@@ -692,6 +705,8 @@ def run_own(args):
     model._begin_fit("sgd")
     P, Q, ws, hp = model.embed_user.weight, model.embed_item.weight, model._ws, model._hp
 
+    last_losses = [None]
+
     def run_steps(first, k, timed):
         """k steps starting at global step `first`, walking the epoch cyclically; one launch per epoch segment."""
         evs, launches, s = [], 0, first
@@ -701,7 +716,7 @@ def run_own(args):
             if timed:
                 e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
                 e0.record()
-            ops.mf_bpr_train_steps(P, Q, ws, bu, bi, bj, B, pos, seg, hp, check=False)
+            last_losses[0] = ops.mf_bpr_train_steps(P, Q, ws, bu, bi, bj, B, pos, seg, hp, check=False)
             if timed:
                 e1.record()
                 evs.append((e0, e1, seg, pos))
@@ -725,6 +740,10 @@ def run_own(args):
     nan_check = ops.mf_bpr_loss(P, Q, ws, bu[:B], bi[:B], bj[:B], hp).item()
     if not np.isfinite(nan_check):
         raise RuntimeError("bench: loss became non-finite during the timed steps")
+    if args.dump_outputs:
+        # what MF.fit's caller holds after the last timed step: both embedding tables and that step's loss
+        dump_outputs(args.dump_outputs, {"embed_user": P.detach().cpu().numpy(), "embed_item": Q.detach().cpu().numpy(),
+                                         "last_step_loss": last_losses[0][-1:].double().cpu().numpy()})
 
     # ---- end to end = the reference's plug-in call (run_examples/test.py:91-95): fit(DataLoader) over PINNED host triples,
     #      one full epoch, wall clock: upload + id check + epoch permutation + gather + all steps + loss read-back
@@ -790,7 +809,8 @@ def run_own(args):
     avg_launch_ms = ms / len(evs)
     avg_launch_triples = done_triples / len(evs)
     achieved = avg_launch_triples * bytes_per_triple / (avg_launch_ms * 1e-3) / 1e9
-    traffic, traffic_src = profiled_traffic(F, B)
+    l2 = torch.cuda.get_device_properties(dev).L2_cache_size
+    work = 2 * (U + I) * F * 4                                       # tables + gradient accumulators
     sk = step_kernel_info(F, U + I)
     line = {"metric": METRIC, "value": value, "unit": UNIT, "n_gpus": 1, "steps": args.steps, "warmup": args.warmup,
             "ms_per_step": ms / args.steps, "higher_is_better": True, "scaling": "weak", "vs_baseline": None,
@@ -811,11 +831,11 @@ def run_own(args):
             "gpu_launches_note": "persistent cooperative kernel: one launch runs up to steps_per_epoch synchronous steps",
             "step_kernel": sk,
             "roofline": {"bound": "hbm", "achieved": achieved, "peak": peak, "unit": "GB/s", "frac": achieved / peak,
-                         "traffic": None if traffic is None else traffic * (args.steps / len(evs)),
-                         "traffic_note": f"dram__bytes_read+write per step ({traffic_src}: ncu capture of the general "
-                                         "instantiation mf_bpr_steps_kernel<4,16,1>; a lean instantiation moves the same rows) x "
-                                         "steps per launch; the 85 MB working set is L2-resident, so the limiter at this shape is "
-                                         "L2/issue, not HBM -- configs.c5_netflix_1gpu is the HBM-regime figure",
+                         "regime_note": f"tables + gradient accumulators {work / 1e6:.0f} MB against this GPU's "
+                                        f"{l2 / 1e6:.0f} MB L2: " + (
+                                            "HBM regime, rows are served partly from L2 and partly from HBM (split not "
+                                            "measured), so the algorithmic GB/s is not a DRAM rate" if work > l2 else
+                                            "L2 regime, the algorithmic GB/s is mostly L2 traffic"),
                          "peak_source": peak_src, "algorithmic_bytes_per_triple": bytes_per_triple,
                          "kernel": sk["instantiation"], "avg_launch_ms": avg_launch_ms},
             "cpu_baseline": cpu,
@@ -1060,7 +1080,12 @@ def main():
     ap.add_argument("--ref-workers", dest="ref_workers", type=int, default=4, help="DataLoader workers of the reference (test.py:94)")
     ap.add_argument("--rows-file", dest="rows_file", default=None, help="reference arm: .npy of sampler triples to train on")
     ap.add_argument("--quick", action="store_true", help="reference arm: main measurement only")
+    ap.add_argument("--dump-outputs", dest="dump_outputs", default=None, metavar="DIR",
+                    help="own arm, one GPU: after the timed steps write the tables and the last step's loss as DIR/<name>.npy "
+                         "(a seeded sample where they exceed 64 MB in all)")
     args = ap.parse_args()
+    if args.dump_outputs and (args.impl == "reference" or args.gpus > 1):
+        ap.error("--dump-outputs writes what the single-GPU own arm computed: it needs --impl own and --gpus 1")
     if args.impl == "reference":
         args.steps = 8 if args.steps is None else args.steps
         args.warmup = 2 if args.warmup is None else args.warmup

@@ -1,4 +1,4 @@
-"""daisyrec_b200 -- B200-native (sm_100a) BPR training / ranking path behind daisyRec's plug-in API.
+"""daisyrec_b200 -- H100-native (sm_90a) BPR training / ranking path behind daisyRec's plug-in API.
 
 Drop-in surface (same names and call signatures as AmazingDD/daisyRec v2.3.0):
     daisyrec_b200.model.MFRecommender.MF                 <- daisy/model/MFRecommender.py

@@ -229,7 +229,7 @@ def lib():
         except Exception as e:  # noqa: BLE001
             raise RuntimeError(
                 f"libdaisyrec_b200.so is missing ({path}) and could not be built: {e}. "
-                "The B200 path has no CPU fallback; run `python -c 'import __graft_entry__ as g; g.build()'`.") from e
+                "The GPU path has no CPU fallback; run `python -c 'import __graft_entry__ as g; g.build()'`.") from e
     L = C.CDLL(path)
     for name, (res, args) in SIGNATURES.items():
         fn = getattr(L, name)          # AttributeError here == header and library out of sync

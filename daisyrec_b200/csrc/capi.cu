@@ -30,10 +30,10 @@ int sm_count()
 {
     static thread_local int cached_dev = -1, cached = 0;
     int dev = 0;
-    if (cudaGetDevice(&dev) != cudaSuccess) return 148;
+    if (cudaGetDevice(&dev) != cudaSuccess) return 132;
     if (dev != cached_dev) {
         cudaDeviceProp prop;
-        if (cudaGetDeviceProperties(&prop, dev) != cudaSuccess) return 148;
+        if (cudaGetDeviceProperties(&prop, dev) != cudaSuccess) return 132;
         cached = prop.multiProcessorCount;
         cached_dev = dev;
     }

@@ -1,4 +1,4 @@
-// gemm.cuh -- plain entry points of the dense-layer GEMM dispatcher in neumf.cu (dtype 0: fp32 CUDA cores, 1: bf16 tcgen05).
+// gemm.cuh -- plain entry points of the dense-layer GEMM dispatcher in neumf.cu (dtype 0: fp32 CUDA cores, 1: bf16 wgmma).
 #pragma once
 #include "common.cuh"
 
@@ -15,5 +15,7 @@ int gemm_tn_acc_t(int dtype, long long M, int N, int K, const float *A, long lon
                   long long ldc, cudaStream_t st);
 // gb[n] += sum_m dZ[m, n]          (bias gradient, N <= 256)
 int colsum_acc(const float *dZ, long long M, int N, float *gb, cudaStream_t st);
+// the same over the 2B rows of a pairwise step, each pos row m added to its neg row B + m first
+int colsum_pairs_acc(const float *dZ, long long B, int N, float *gb, cudaStream_t st);
 
 }  // namespace drb

@@ -1,4 +1,4 @@
-// lightgcn.cu -- LightGCN + BPR on the B200 path (SURVEY 8(a) row a15).
+// lightgcn.cu -- LightGCN + BPR on the GPU path (SURVEY 8(a) row a15).
 //
 // Stands behind daisy/model/LightGCNRecommender.py:
 //   forward   :117-129   E_l = A_hat E_{l-1} (torch.sparse.mm, :122), mean over the L+1 layers

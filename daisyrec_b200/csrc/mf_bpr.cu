@@ -1,4 +1,4 @@
-// mf_bpr.cu -- the BPR-MF training step as ONE persistent cooperative sm_100a kernel.
+// mf_bpr.cu -- the BPR-MF training step as ONE persistent cooperative sm_90a kernel.
 //
 // Stands behind GeneralRecommender.fit's step loop (daisy/model/AbstractRecommender.py:112-128)
 // with MF.calc_loss (daisy/model/MFRecommender.py:70-97), BPRLoss (daisy/utils/loss.py:11),
@@ -284,10 +284,24 @@ static bool same_results(const CheckProblem &c, int opt, const std::vector<float
     return ok && moved > 1e-4;                                   // and the steps did move the tables
 }
 
-// The lean instantiations were written after the last GPU slot of their round, so nothing about them is assumed: once per
-// process and factor count every candidate geometry (1) must reproduce the general instantiation on a small seeded problem
-// (two SGD and two Adam steps), and (2) is timed against it on an L2-regime problem with the bench's index statistics
-// (3 steps x 524 288 triples, best of two warm launches).  The fastest correct candidate is used if it beats the general
+// L2 size of the current device (the regime test and the L2-regime timing problem are sized from it)
+static long long l2_bytes()
+{
+    static const long long l2 = [] {
+        int dev = 0, bytes = 0;
+        if (cudaGetDevice(&dev) != cudaSuccess || cudaDeviceGetAttribute(&bytes, cudaDevAttrL2CacheSize, dev) != cudaSuccess) {
+            cudaGetLastError();
+            bytes = 0;
+        }
+        return (long long)(bytes > 0 ? bytes : 64 << 20);
+    }();
+    return l2;
+}
+
+// Nothing about the speed of the lean instantiations is assumed: once per process, factor count and regime every candidate
+// geometry (1) must reproduce the general instantiation on a small seeded problem (two SGD and two Adam steps), and (2) is
+// timed against it on a problem of the caller's regime with the bench's index statistics (3 steps x 524 288 triples, best of
+// two warm launches).  The fastest correct candidate is used if it beats the general
 // instantiation, and a larger index tile if that helps it further; otherwise the general kernel stays.  Never a wrong table,
 // never a slower step.
 static LeanChoice lean_autotune(int F, bool hbm)
@@ -299,8 +313,10 @@ static LeanChoice lean_autotune(int F, bool hbm)
     if (gen == nullptr || ncand == 0) return best;
     CheckProblem small, big;
     make_check_problem(small, 96, 80, F, 384, 2, true);
-    // timing problem: tables + accumulators inside L2 (like BASELINE config 2) or, for the HBM regime, 2 x 134 MB of user rows
-    const int rows = hbm ? 33554432 / F : (F <= 64 ? 131072 : 65536);
+    // timing problem: for the L2 regime U = 4 I rows whose tables + accumulators take half of this device's L2 (the other half is
+    // left to the streamed index planes); for the HBM regime 2 x 134 MB of user rows
+    const long long l2_rows = l2_bytes() / (2LL * 8 * F) * 4 / 5;
+    const int rows = hbm ? 33554432 / F : (int)(l2_rows > 4096 ? l2_rows : 4096);
     make_check_problem(big, rows, hbm ? 16384 : rows / 4, F, 1 << 19, 3, false);
     std::vector<float> refP[2], refQ[2];
     double refl[2][2];
@@ -351,15 +367,7 @@ static LeanChoice lean_autotune(int F, bool hbm)
 // regime of a problem: do the two tables and their accumulators fit the L2 cache?
 static bool hbm_regime(long long table_rows, int F)
 {
-    static const long long l2 = [] {
-        int dev = 0, bytes = 0;
-        if (cudaGetDevice(&dev) != cudaSuccess || cudaDeviceGetAttribute(&bytes, cudaDevAttrL2CacheSize, dev) != cudaSuccess) {
-            cudaGetLastError();
-            bytes = 0;
-        }
-        return (long long)(bytes > 0 ? bytes : 64 << 20);
-    }();
-    return table_rows * (long long)F * 8 > l2;
+    return table_rows * (long long)F * 8 > l2_bytes();
 }
 
 static const LeanChoice &lean_choice(int F, long long table_rows)

@@ -1,4 +1,4 @@
-// neumf.cu -- NeuMF + BPR on the B200 path (SURVEY 8(a) row a14), fp32 tower on CUDA cores.
+// neumf.cu -- NeuMF + BPR on the GPU path (SURVEY 8(a) row a14), fp32 tower on CUDA cores.
 //
 // Stands behind daisy/model/NeuMFRecommender.py (model_name == 'NeuMF'):
 //   forward   :118-137  GMF = UG[u]*IG[i];  x0 = cat(UM[u], IM[i]);  L x (Dropout -> Linear -> ReLU);  Linear(2F, 1)
@@ -18,7 +18,7 @@
 //
 // Rooflines: the tower is ~124 KFLOP per triple at F=32, L=2 (fwd+bwd, both items) against ~2.3 KB of embedding traffic:
 // compute-bound on CUDA cores in the fp32 path (tower_dtype 0); with tower_dtype 1 the three GEMM call sites run on
-// tcgen05 (umma_gemm.cuh) and the step becomes bound by streaming the fp32 activations (profiles/r01c).
+// wgmma tensor cores (umma_gemm.cuh) and the step becomes bound by streaming the fp32 activations.
 #include "step.cuh"
 #include "umma_gemm.cuh"
 #include "neumf_fused.cuh"
@@ -195,7 +195,7 @@ static int launch_sgemm(long long M, int N, int K, const float *A, long long lda
     return DRB_OK;
 }
 
-// dtype 0: fp32 CUDA cores (sgemm_kernel)   dtype 1: bf16 operands on tcgen05 tensor cores, fp32 accumulate in TMEM
+// dtype 0: fp32 CUDA cores (sgemm_kernel)   dtype 1: bf16 operands on wgmma tensor cores, fp32 accumulate in registers
 template <bool TA, bool TB, int EPI>
 static int launch_gemm(int dtype, long long M, int N, int K, const float *A, long long lda, const float *B, long long ldb,
                        float *C, long long ldc, const float *bias, const float *ref, long long ldref, cudaStream_t st,
@@ -441,6 +441,28 @@ __global__ void __launch_bounds__(256) colsum_kernel(const float *__restrict__ d
     }
 }
 
+// gb[n] += sum_{m < B} (dZ[m, n] + dZ[B + m, n]) over the 2B rows of a pairwise step (pos rows [0, B), neg rows [B, 2B)).
+// Each pos row is added to its own neg row first: where a unit is active on both rows of every triple, d pred_neg = -d pred_pos
+// makes every pair cancel exactly and the bias gradient is exactly 0, as in the reference; a row-blocked sum would leave a
+// rounding residual there, which Adam turns into a full lr step.
+__global__ void __launch_bounds__(256) colsum_pairs_kernel(const float *__restrict__ dZ, long long B, int N, float *__restrict__ gb)
+{
+    __shared__ float s_part[256];
+    const int rows_per_pass = 256 / N > 0 ? 256 / N : 1;       // N <= 256
+    const int tr = threadIdx.x / N, tn = threadIdx.x % N;
+    float s = 0.f;
+    if (tr < rows_per_pass)
+        for (long long m = (long long)blockIdx.x * rows_per_pass + tr; m < B; m += (long long)gridDim.x * rows_per_pass)
+            s += dZ[m * N + tn] + dZ[(m + B) * N + tn];
+    s_part[threadIdx.x] = (tr < rows_per_pass) ? s : 0.f;
+    __syncthreads();
+    if (threadIdx.x < N) {
+        float t = 0.f;
+        for (int q = 0; q < rows_per_pass; ++q) t += s_part[q * N + threadIdx.x];
+        if (t != 0.f) atomicAdd(gb + threadIdx.x, t);
+    }
+}
+
 // gUM[u] += dA0[t,:D] + dA0[B+t,:D];  gIM[i] += dA0[t,D:];  gIM[j] += dA0[B+t,D:]      (RED.ADD.F32x4)
 __global__ void neumf_scatter_kernel(const float *__restrict__ dA0, const int32_t *__restrict__ bu,
                                      const int32_t *__restrict__ bi, const int32_t *__restrict__ bj, long long B, int D,
@@ -570,6 +592,15 @@ int colsum_acc(const float *dZ, long long M, int N, float *gb, cudaStream_t st)
     return DRB_OK;
 }
 
+int colsum_pairs_acc(const float *dZ, long long B, int N, float *gb, cudaStream_t st)
+{
+    DRB_REQUIRE(N <= 256, "colsum: N=%d exceeds 256", N);
+    if (B <= 0) return DRB_OK;
+    colsum_pairs_kernel<<<sm_count() * 4, 256, 0, st>>>(dZ, B, N, gb);
+    DRB_CUDA(cudaGetLastError());
+    return DRB_OK;
+}
+
 static int grid1d(long long n, int block, int per_sm = 16)
 {
     long long b = (n + block - 1) / block, cap = (long long)sm_count() * per_sm;
@@ -649,7 +680,7 @@ extern "C" int drb_neumf_bpr_train_steps(float *d_UG, float *d_IG, float *d_UM, 
 {
     NeumfDims d, dlay;
     DRB_REQUIRE(tower_dtype >= 0 && tower_dtype <= 2,
-                "neumf: tower_dtype must be 0 (fp32), 1 (bf16 tcgen05, layer-wise) or 2 (bf16 tcgen05, fused per tile)");
+                "neumf: tower_dtype must be 0 (fp32), 1 (bf16 wgmma, layer-wise) or 2 (bf16 wgmma, fused per tile)");
     DRB_REQUIRE(dropout >= 0.f && dropout < 1.f, "neumf: dropout must be in [0, 1)");
     const bool fused = tower_dtype == 2 && neumf_fused_supported(F, L, mode, dropout);
     if (tower_dtype == 2 && !fused) tower_dtype = 1;      // shapes outside the fused kernel: same numerics class, layer-wise
@@ -726,7 +757,7 @@ extern "C" int drb_neumf_bpr_train_steps(float *d_UG, float *d_IG, float *d_UM, 
         for (int l = d.L - 1; l >= 0 && use_tower && !fused; --l) {
             const float *Aprev = w.acts + d.act_off[l] * R;
             // gW_l[out,in] += dZ^T A_{l-1}, computed as (A_{l-1}^T dZ)^T: the wide dimension (in) fills the 128-row MMA tile
-            // and the narrow one (out) becomes N, so the TMEM footprint per CTA is small and more CTAs overlap
+            // and the narrow one (out) becomes N, so the accumulator footprint per CTA is small and more CTAs overlap
             // (split-K over the R rows; transposed atomic accumulate into gW_l)
             rc = launch_gemm<true, false, 4>(tower_dtype, d.n[l], d.n[l + 1], (int)R, Aprev, d.n[l], cur, d.n[l + 1], w.gW + d.w_off[l],
                                               d.n[l], nullptr, nullptr, 0, st);

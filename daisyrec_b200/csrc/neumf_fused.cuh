@@ -3,23 +3,25 @@
 // Stands behind NeuMF.forward / calc_loss / backward (daisy/model/NeuMFRecommender.py:118-169) for model_name 'NeuMF',
 // num_layers = 2, factors = 32, dropout 0 (BASELINE config 3: F = 32, tower 128 -> 64 -> 32).  The layer-wise
 // path (neumf.cu: gather, 2 forward GEMMs, head, 4 backward GEMMs, 2 column sums, scatter) streams fp32 activations through
-// HBM between ~12 launches (profiles/r01c: 10 % of the HBM roofline).  Here one persistent CTA per SM walks tiles of 64
-// triples = 128 rows (rows 0..63 the pos items, 64..127 the neg items of the same triples):
+// HBM between ~12 launches.  Here one persistent CTA per SM (four warpgroups) walks tiles of 64 triples = 128 rows
+// (rows 0..63 the pos items, 64..127 the neg items of the same triples):
 //
 //   gather   A0 = cat(UM[u], IM[item]) rounded to bf16 straight into the K-major core-matrix image the tensor core reads
 //            (lane group per row, 128-bit loads; the user row is loaded once and stored for both of its tile rows)
-//   MMA      Z1 = A0 W1^T  -> TMEM            tcgen05.mma kind::f16, M = 128, fp32 accumulate
-//   epilogue A1 = relu(Z1 + b1) -> bf16 image (tcgen05.ld, thread = tile row)
-//   MMA      Z2 = A1 W2^T  -> TMEM
+//   MMA      Z1 = A0 W1^T                      wgmma m64nNk16 bf16, fp32 accumulators in registers
+//   epilogue A1 = relu(Z1 + b1) -> bf16 image (straight from the accumulator fragment)
+//   MMA      Z2 = A1 W2^T
 //   head     h = relu(Z2 + b2);  pred = wp . cat(UG[u] * IG[item], h) + bp;  x = pred_pos - pred_neg (rows r and r + 64 meet
-//            through shared memory);  c = BPR coefficient;  loss / regulariser norms;  GMF-table gradients by RED.128;
+//            through shared memory);  c = BPR coefficient;  loss / regulariser norms;  GMF-table gradients by RED;
 //            dZ2 = +-c wp_h [h > 0] -> bf16 image
-//   MMA      dA1 = dZ2 W2  -> TMEM;   gW2^T += A1^T dZ2  -> TMEM (accumulated over ALL tiles of the CTA)
+//   MMA      dA1 = dZ2 W2;   gW2^T += A1^T dZ2  (register accumulators carried over ALL tiles of the CTA)
 //   epilogue dZ1 = dA1 [A1 > 0] -> bf16 image
-//   MMA      dA0 = dZ1 W1  -> TMEM;   gW1^T += A0^T dZ1  -> TMEM (accumulated over all tiles)
+//   MMA      dA0 = dZ1 W1;   gW1^T += A0^T dZ1  (carried over all tiles)
 //   epilogue dA0 -> RED.128 into gUM[u] / gIM[item]
-//   finally  the two weight gradients leave TMEM once per CTA; bias / predict-layer gradients, loss and norms are carried in
-//            registers across tiles and reduced once.
+//   finally  the two weight gradients leave the registers once per CTA; bias / predict-layer gradients, loss and norms are
+//            carried in registers across tiles and reduced once.
+// Every product is split over the four warpgroups: warpgroup g takes row half (g & 1) -- or, for the A^T dZ products, K half
+// or feature half -- and column half (g >> 1), so each issues m64n32 / m64n16 MMAs on its own accumulators.
 // Every activation / gradient tile is written ONCE as a K-major operand image (element (row, k) at
 // (k/8) LBO + (row/8) 128 + (row%8) 16 + (k%8) 2).  The same bytes are the MN-major image of the TRANSPOSED tile when the
 // descriptor's two strides are swapped (K-group stride 128, MN-group stride LBO), which is how A^T dZ and dZ W are fed
@@ -29,7 +31,7 @@
 
 namespace drb {
 
-constexpr int kFusedThreads = 512;      // 16 warps: TMEM lane quarter = warp % 4, column quarter = warp / 4
+constexpr int kFusedThreads = 512;      // 4 warpgroups: row (or K / feature) half = g & 1, column half = g >> 1
 constexpr int kFusedTile = 64;          // triples per tile (128 rows)
 
 struct FusedParams {
@@ -58,102 +60,53 @@ struct FusedLayout {
     static constexpr uint32_t W1 = DZ2 + (N2 / 8) * LBO_T;
     static constexpr uint32_t W2 = W1 + (N0 / 8) * LBO_W1;
     static constexpr uint32_t W_END = W2 + (N1 / 8) * LBO_W2;
-    // fp32 staging of the NEXT tile's gathered rows (cp.async): MLP rows [3][64][D], GMF rows [3][64][F + 4] (padded: the head
-    // reads one row per lane with 128-bit loads)
+    // fp32 staging of the NEXT tile's gathered rows (cp.async): MLP rows [3][64][D], GMF rows [3][64][F + 4] (padded)
     static constexpr uint32_t SM = (W_END + 127) / 128 * 128;
     static constexpr uint32_t SG = SM + 3 * 64 * D * 4;
     static constexpr int GROW = F + 4;
     static constexpr uint32_t TAIL = SG + 3 * 64 * GROW * 4;
-    // the gW2 product reads A1^T as an M = 128 operand although only N1 <= 96 feature rows exist: MN-groups beyond N1/8 fall
-    // into the images behind A1 (finite bf16 data, rows of the result that nobody reads) -- keep that window inside the buffer
-    static constexpr uint32_t SPAN = (A1 + 16 * LBO_T + 256 > TAIL) ? (A1 + 16 * LBO_T + 256) : TAIL;
-    static constexpr uint32_t BYTES = (SPAN + 127) / 128 * 128;
-    // TMEM columns
-    static constexpr int C_Z1 = 0, C_Z2 = N1, C_DA0 = 128, C_GW2 = 128 + N0, C_GW1 = 128 + N0 + 32 * ((N2 + 31) / 32);
-    static constexpr int C_END = C_GW1 + N1;
-    static_assert(N1 + N2 <= 128 && C_END <= 512, "TMEM budget");
+    static constexpr uint32_t BYTES = (TAIL + 127) / 128 * 128;
 };
 
-__device__ __forceinline__ void fused_mma(uint32_t tmem_d, uint64_t da, uint64_t db, uint32_t idesc, uint32_t accumulate)
+// bf16 pair (k, k + 1), k even, of tile row `row` of a K-major image with 128 rows: one 4-byte store
+__device__ __forceinline__ uint32_t image_off(uint32_t lbo, int row, int k)
 {
-    asm volatile(
-        "{\n\t"
-        ".reg .pred p;\n\t"
-        "setp.ne.b32 p, %4, 0;\n\t"
-        "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t"
-        "}\n" ::"r"(tmem_d),
-        "l"(da), "l"(db), "r"(idesc), "r"(accumulate)
-        : "memory");
+    return (uint32_t)(k >> 3) * lbo + (uint32_t)(row >> 3) * 128u + (uint32_t)(row & 7) * 16u + (uint32_t)(k & 7) * 2u;
 }
-__device__ __forceinline__ void fused_commit(uint64_t *bar)
+__device__ __forceinline__ void image_store2(unsigned char *img, uint32_t lbo, int row, int k, float a, float b)
 {
-    asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(smem_u32(bar)) : "memory");
+    *reinterpret_cast<uint32_t *>(img + image_off(lbo, row, k)) = pack_bf16x2(a, b);
 }
-// 16 / 8 consecutive fp32 columns of this warp's 32 TMEM lanes (thread = lane = tile row); the caller waits (tmem_wait)
-__device__ __forceinline__ void tmem_ld16_nowait(uint32_t taddr, uint32_t (&r)[16])
-{
-    asm volatile(
-        "tcgen05.ld.sync.aligned.32x32b.x16.b32 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, [%16];"
-        : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]), "=r"(r[9]),
-          "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15])
-        : "r"(taddr));
-}
-__device__ __forceinline__ void tmem_ld8_nowait(uint32_t taddr, uint32_t (&r)[8])
-{
-    asm volatile("tcgen05.ld.sync.aligned.32x32b.x8.b32 {%0, %1, %2, %3, %4, %5, %6, %7}, [%8];"
-                 : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7])
-                 : "r"(taddr));
-}
-__device__ __forceinline__ void tmem_wait() { asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory"); }
-
-// 8 bf16 (k0 .. k0+7, k0 % 8 == 0) of tile row `row` of a K-major image with 128 rows: one 16-byte store
-__device__ __forceinline__ void image_store8(unsigned char *img, uint32_t lbo, int row, int k0, const float *v)
-{
-    uint4 a;
-    a.x = pack_bf16x2(v[0], v[1]); a.y = pack_bf16x2(v[2], v[3]); a.z = pack_bf16x2(v[4], v[5]); a.w = pack_bf16x2(v[6], v[7]);
-    *reinterpret_cast<uint4 *>(img + (uint32_t)(k0 >> 3) * lbo + (uint32_t)(row >> 3) * 128u + (uint32_t)(row & 7) * 16u) = a;
-}
+__device__ __forceinline__ bool bf16_positive(uint32_t hbits) { return (hbits & 0x7fffu) != 0u && (hbits & 0x8000u) == 0u; }
 
 template <int F>
 __global__ void __launch_bounds__(kFusedThreads, 1) neumf_fused_kernel(FusedParams p)
 {
     using L = FusedLayout<F>;
     constexpr int D = L::D, N0 = L::N0, N1 = L::N1, N2 = L::N2;
-    constexpr int NP = 4;                         // column parts: every TMEM tile is split over warp / 4
-    constexpr int C1 = N1 / NP, C2 = N2 / NP, CG = F / NP, C0 = N0 / NP;   // columns per thread: Z1/dA1, Z2, GMF, dA0
-    static_assert(C1 == 16 && C2 == 8 && CG == 8 && C0 == 32, "the epilogues are written for factors = 32");
+    static_assert(N0 == 128 && N1 == 64 && N2 == 32, "the warpgroup split is written for factors = 32");
     extern __shared__ __align__(128) unsigned char smem[];
-    __shared__ __align__(8) uint64_t s_bar;
-    __shared__ uint32_t s_tmem;
     __shared__ float s_b1[N1], s_b2[N2], s_wp[2 * F + 1];
-    __shared__ float s_pred[NP][128];
+    __shared__ float s_pred[2][128];
     __shared__ int s_idx[2][3][kFusedTile];       // [buffer][u | i | j][triple] of the current and the next tile
     __shared__ float s_colsum[N1 + N2 + 2 * F];   // final cross-thread reduction of the register column sums
     __shared__ double s_red[11];
 
     const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
-    const int q = warp & 3, part = warp >> 2;     // TMEM lane quarter of this warp, column quarter it works on
-    const int row = q * 32 + lane;                // tile row owned in every epilogue (4 threads share it)
-    const bool pos_row = row < kFusedTile;
+    const int wg = tid >> 7, mh = wg & 1, nh = wg >> 1;     // row (K, feature) half and column half of this warpgroup
+    const int quad = lane & 3;
+    const int rbase = mh * 64 + (warp & 3) * 16 + (lane >> 2);   // fragment rows rbase and rbase + 8
+    const bool pos_row = mh == 0;                            // rows 0..63: pos items, 64..127: neg items
     const float sign = pos_row ? 1.f : -1.f;
 
-    // ---- one-off: TMEM, barrier, weights as bf16 operand images, biases
-    if (warp == 0) {
-        asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(&s_tmem)), "r"(512) : "memory");
-        asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-    }
-    if (tid == 0) {
-        mbar_init(&s_bar, 1);
-        fence_mbar_init();
-    }
+    // ---- one-off: weights as bf16 operand images, biases
     const float *W1 = p.W, *b1 = W1 + (size_t)N1 * N0, *W2 = b1 + N1, *b2 = W2 + (size_t)N2 * N1, *wp = b2 + N2;
     for (int it = tid; it < N1 * (N0 / 8); it += kFusedThreads) {            // W1 [N1 rows, N0 k] K-major image
         const int r = it / (N0 / 8), kg = it % (N0 / 8);
         const float4 *s4 = reinterpret_cast<const float4 *>(W1 + (size_t)r * N0 + kg * 8);
         const float4 a = __ldg(s4), b = __ldg(s4 + 1);
-        const float v[8] = {a.x, a.y, a.z, a.w, b.x, b.y, b.z, b.w};
         uint4 o;
-        o.x = pack_bf16x2(v[0], v[1]); o.y = pack_bf16x2(v[2], v[3]); o.z = pack_bf16x2(v[4], v[5]); o.w = pack_bf16x2(v[6], v[7]);
+        o.x = pack_bf16x2(a.x, a.y); o.y = pack_bf16x2(a.z, a.w); o.z = pack_bf16x2(b.x, b.y); o.w = pack_bf16x2(b.z, b.w);
         *reinterpret_cast<uint4 *>(smem + L::W1 + (uint32_t)kg * L::LBO_W1 + (uint32_t)(r >> 3) * 128u + (uint32_t)(r & 7) * 16u) = o;
     }
     for (int it = tid; it < N2 * (N1 / 8); it += kFusedThreads) {            // W2 [N2 rows, N1 k]
@@ -169,27 +122,19 @@ __global__ void __launch_bounds__(kFusedThreads, 1) neumf_fused_kernel(FusedPara
     for (int k = tid; k < 2 * F + 1; k += kFusedThreads) s_wp[k] = wp[k];
     if (tid < 11) s_red[tid] = 0.0;
     for (int k = tid; k < N1 + N2 + 2 * F; k += kFusedThreads) s_colsum[k] = 0.f;
-    // the windows the padded M = 128 views may touch must hold finite numbers before the first product reads them
-    for (uint32_t o = L::DZ1 + tid * 16u; o < L::W1; o += kFusedThreads * 16u) *reinterpret_cast<uint4 *>(smem + o) = make_uint4(0, 0, 0, 0);
-    tc_fence_before();
     __syncthreads();
-    tc_fence_after();
-    const uint32_t tmem = s_tmem;
     const uint32_t sbase = smem_u32(smem);
-    const uint32_t taddr = tmem + ((uint32_t)(q * 32) << 16);          // this warp's TMEM lanes
-    uint32_t phase = 0;
 
     // register accumulators carried across tiles (reduced once at the end)
     float acc_loss = 0.f, acc_l1[5] = {0, 0, 0, 0, 0}, acc_s2[5] = {0, 0, 0, 0, 0};
-    float gb1[C1], gb2[C2], gwg[CG], gwh[C2];
+    float gw1[16], gw2[8];                        // gW1^T [features of half mh] x [outputs of half nh]; gW2^T K-half mh
+    float gb1[8], gb2[4], gwg[4], gwh[4];         // column sums of this thread's fragment columns
 #pragma unroll
-    for (int k = 0; k < C1; ++k) gb1[k] = 0.f;
+    for (int k = 0; k < 16; ++k) gw1[k] = 0.f;
 #pragma unroll
-    for (int k = 0; k < C2; ++k) { gb2[k] = 0.f; gwh[k] = 0.f; }
+    for (int k = 0; k < 8; ++k) { gw2[k] = 0.f; gb1[k] = 0.f; }
 #pragma unroll
-    for (int k = 0; k < CG; ++k) gwg[k] = 0.f;
-
-    auto idesc = [&](int N, bool a_mn, bool b_mn) { return umma_idesc_bf16_f32(128, N, a_mn, b_mn); };
+    for (int k = 0; k < 4; ++k) { gb2[k] = 0.f; gwg[k] = 0.f; gwh[k] = 0.f; }
 
     const long long ntiles = (p.B + kFusedTile - 1) / kFusedTile;
     bool first_tile = true;
@@ -254,15 +199,20 @@ __global__ void __launch_bounds__(kFusedThreads, 1) neumf_fused_kernel(FusedPara
     for (long long tile = blockIdx.x; tile < ntiles; tile += gridDim.x, cur ^= 1) {
         const long long t0 = tile * kFusedTile;
         const int nt = (int)min((long long)kFusedTile, p.B - t0);           // valid triples in this tile
-        const int tr = row & (kFusedTile - 1);                              // triple of this thread's row
-        const bool ok = tr < nt;
         const long long next_tile = tile + gridDim.x;
         const bool has_next = next_tile < ntiles;
         const int idx_next = has_next ? fetch_index(next_tile) : 0;        // lands while this tile's rows are converted
         asm volatile("cp.async.wait_group 0;" ::: "memory");
         __syncthreads();                                                    // staged rows of this tile visible to everyone
-        const int u = s_idx[cur][0][tr];
-        const int item = s_idx[cur][pos_row ? 1 : 2][tr];
+        int trr[2], uu[2], itm[2];
+        bool ok[2];
+#pragma unroll
+        for (int i = 0; i < 2; ++i) {
+            trr[i] = (rbase + 8 * i) & (kFusedTile - 1);                    // triple of fragment row i
+            ok[i] = trr[i] < nt;
+            uu[i] = s_idx[cur][0][trr[i]];
+            itm[i] = s_idx[cur][pos_row ? 1 : 2][trr[i]];
+        }
 
         // ---------------------------------------------------------------- A0: staged fp32 rows -> bf16 K-major image
         {
@@ -281,8 +231,7 @@ __global__ void __launch_bounds__(kFusedThreads, 1) neumf_fused_kernel(FusedPara
                 o.y = pack_bf16x2(v.z, v.w);
                 const int k = (kind == 0 ? 0 : D) + gl * 4;
                 const int trow = kind == 2 ? r + kFusedTile : r;
-                const uint32_t off = L::A0 + (uint32_t)(k >> 3) * L::LBO_T + (uint32_t)(trow >> 3) * 128u + (uint32_t)(trow & 7) * 16u +
-                                     (uint32_t)(k & 7) * 2u;
+                const uint32_t off = L::A0 + image_off(L::LBO_T, trow, k);
                 *reinterpret_cast<uint2 *>(smem + off) = o;
                 if (kind == 0) *reinterpret_cast<uint2 *>(smem + off + (kFusedTile >> 3) * 128u) = o;   // the neg row of the triple
             }
@@ -291,141 +240,130 @@ __global__ void __launch_bounds__(kFusedThreads, 1) neumf_fused_kernel(FusedPara
         asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
         __syncthreads();
 
-        // ---------------------------------------------------------------- Z1 = A0 W1^T
-        if (tid == 0) {
-            tc_fence_after();
-            const uint32_t id = idesc(N1, false, false);
+        // ---------------------------------------------------------------- Z1 = A0 W1^T  (rows of half mh, columns of half nh)
+        float z1[16];
 #pragma unroll
-            for (int kk = 0; kk < N0 / 16; ++kk)
-                fused_mma(tmem + L::C_Z1, umma_smem_desc(sbase + L::A0 + kk * 2 * L::LBO_T, L::LBO_T, 128),
-                          umma_smem_desc(sbase + L::W1 + kk * 2 * L::LBO_W1, L::LBO_W1, 128), id, kk > 0);
-            fused_commit(&s_bar);
-        }
+        for (int e = 0; e < 16; ++e) z1[e] = 0.f;
+        wgmma_fence();
+#pragma unroll
+        for (int kk = 0; kk < N0 / 16; ++kk)
+            wgmma_m64n32<0, 0>(z1, umma_smem_desc(sbase + L::A0 + mh * 1024 + kk * 2 * L::LBO_T, L::LBO_T, 128),
+                               umma_smem_desc(sbase + L::W1 + nh * 512 + kk * 2 * L::LBO_W1, L::LBO_W1, 128), kk > 0);
+        wgmma_commit();
         if (has_next) prefetch_mlp(next_tile, cur ^ 1);      // the MLP staging has been consumed: refill it under the MMAs
-        mbar_wait(&s_bar, phase);
-        phase ^= 1;
-        tc_fence_after();
+        wgmma_wait_all();
+        wgmma_fence_operand(z1);
 
         // ---------------------------------------------------------------- A1 = relu(Z1 + b1) -> image
-        {
-            const int k0 = part * C1;
-            uint32_t r16[16];
-            tmem_ld16_nowait(taddr + (uint32_t)(L::C_Z1 + k0), r16);
-            tmem_wait();
-            float v[16];
 #pragma unroll
-            for (int e = 0; e < 16; ++e) {
-                const float z = __uint_as_float(r16[e]) + s_b1[k0 + e];
-                v[e] = (ok && z > 0.f) ? z : 0.f;
+        for (int nb = 0; nb < 4; ++nb) {
+            const int col = nh * 32 + nb * 8 + 2 * quad;
+#pragma unroll
+            for (int i = 0; i < 2; ++i) {
+                const float za = z1[nb * 4 + 2 * i] + s_b1[col], zb = z1[nb * 4 + 2 * i + 1] + s_b1[col + 1];
+                image_store2(smem + L::A1, L::LBO_T, rbase + 8 * i, col, (ok[i] && za > 0.f) ? za : 0.f,
+                             (ok[i] && zb > 0.f) ? zb : 0.f);
             }
-            image_store8(smem + L::A1, L::LBO_T, row, k0, v);
-            image_store8(smem + L::A1, L::LBO_T, row, k0 + 8, v + 8);
         }
-        tc_fence_before();
         asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
         __syncthreads();
 
-        // ---------------------------------------------------------------- Z2 = A1 W2^T
-        if (tid == 0) {
-            tc_fence_after();
-            const uint32_t id = idesc(N2, false, false);
+        // ---------------------------------------------------------------- Z2 = A1 W2^T  (rows of half mh, 16 columns of half nh)
+        float z2[8];
 #pragma unroll
-            for (int kk = 0; kk < N1 / 16; ++kk)
-                fused_mma(tmem + L::C_Z2, umma_smem_desc(sbase + L::A1 + kk * 2 * L::LBO_T, L::LBO_T, 128),
-                          umma_smem_desc(sbase + L::W2 + kk * 2 * L::LBO_W2, L::LBO_W2, 128), id, kk > 0);
-            fused_commit(&s_bar);
-        }
-        // GMF rows of this thread's 8 columns (shared memory staging; rows beyond the batch were staged as zeros)
-        float gu[CG], gi[CG];
-        {
-            const int k0 = part * CG;
-            const float4 *ug4 = reinterpret_cast<const float4 *>(smem + L::SG + (uint32_t)((0 * kFusedTile + tr) * L::GROW + k0) * 4u);
-            const float4 *ig4 =
-                reinterpret_cast<const float4 *>(smem + L::SG + (uint32_t)(((pos_row ? 1 : 2) * kFusedTile + tr) * L::GROW + k0) * 4u);
+        for (int e = 0; e < 8; ++e) z2[e] = 0.f;
+        wgmma_fence();
 #pragma unroll
-            for (int c = 0; c < CG / 4; ++c) {
-                const float4 a = ug4[c], b = ig4[c];
-                gu[4 * c] = a.x; gu[4 * c + 1] = a.y; gu[4 * c + 2] = a.z; gu[4 * c + 3] = a.w;
-                gi[4 * c] = b.x; gi[4 * c + 1] = b.y; gi[4 * c + 2] = b.z; gi[4 * c + 3] = b.w;
+        for (int kk = 0; kk < N1 / 16; ++kk)
+            wgmma_m64n16<0, 0>(z2, umma_smem_desc(sbase + L::A1 + mh * 1024 + kk * 2 * L::LBO_T, L::LBO_T, 128),
+                               umma_smem_desc(sbase + L::W2 + nh * 256 + kk * 2 * L::LBO_W2, L::LBO_W2, 128), kk > 0);
+        wgmma_commit();
+        // GMF rows at this thread's columns 16 nh + 8 nb + 2 quad + {0, 1} (rows beyond the batch were staged as zeros)
+        float gu[2][4], gi[2][4];
+#pragma unroll
+        for (int i = 0; i < 2; ++i)
+#pragma unroll
+            for (int nb = 0; nb < 2; ++nb) {
+                const int col = nh * 16 + nb * 8 + 2 * quad;
+                const float2 a = *reinterpret_cast<const float2 *>(smem + L::SG + (uint32_t)((0 * kFusedTile + trr[i]) * L::GROW + col) * 4u);
+                const float2 b = *reinterpret_cast<const float2 *>(
+                    smem + L::SG + (uint32_t)(((pos_row ? 1 : 2) * kFusedTile + trr[i]) * L::GROW + col) * 4u);
+                gu[i][2 * nb] = a.x; gu[i][2 * nb + 1] = a.y;
+                gi[i][2 * nb] = b.x; gi[i][2 * nb + 1] = b.y;
             }
-        }
-        mbar_wait(&s_bar, phase);
-        phase ^= 1;
-        tc_fence_after();
+        wgmma_wait_all();
+        wgmma_fence_operand(z2);
 
         // ---------------------------------------------------------------- head: h, prediction, BPR coefficient, dZ2, GMF gradients
-        float hval[C2];
-        {
-            const int k0 = part * C2;
-            uint32_t r8[8];
-            tmem_ld8_nowait(taddr + (uint32_t)(L::C_Z2 + k0), r8);
-            tmem_wait();
+        float hval[2][4];
+#pragma unroll
+        for (int i = 0; i < 2; ++i) {
             float part_sum = 0.f;
 #pragma unroll
-            for (int e = 0; e < C2; ++e) {
-                const float z = __uint_as_float(r8[e]) + s_b2[k0 + e];
-                hval[e] = (ok && z > 0.f) ? z : 0.f;
-                part_sum = fmaf(s_wp[F + k0 + e], hval[e], part_sum);
+            for (int e = 0; e < 4; ++e) {
+                const int col = nh * 16 + (e >> 1) * 8 + 2 * quad + (e & 1);
+                const float z = z2[(e >> 1) * 4 + 2 * i + (e & 1)] + s_b2[col];
+                hval[i][e] = (ok[i] && z > 0.f) ? z : 0.f;
+                part_sum = fmaf(s_wp[F + col], hval[i][e], part_sum);
+                part_sum = fmaf(s_wp[col], gu[i][e] * gi[i][e], part_sum);
             }
-#pragma unroll
-            for (int e = 0; e < CG; ++e) part_sum = fmaf(s_wp[part * CG + e], gu[e] * gi[e], part_sum);
-            s_pred[part][row] = part_sum;
-            if (p.has_reg && ok) {
+            part_sum += __shfl_xor_sync(0xffffffffu, part_sum, 1);
+            part_sum += __shfl_xor_sync(0xffffffffu, part_sum, 2);
+            if (quad == 0) s_pred[nh][rbase + 8 * i] = part_sum;
+            if (p.has_reg && ok[i]) {
                 float a1 = 0.f, q1 = 0.f, a2 = 0.f, q2 = 0.f;
 #pragma unroll
-                for (int e = 0; e < CG; ++e) {
-                    a1 += fabsf(gu[e]); q1 = fmaf(gu[e], gu[e], q1);
-                    a2 += fabsf(gi[e]); q2 = fmaf(gi[e], gi[e], q2);
+                for (int e = 0; e < 4; ++e) {
+                    a1 += fabsf(gu[i][e]); q1 = fmaf(gu[i][e], gu[i][e], q1);
+                    a2 += fabsf(gi[i][e]); q2 = fmaf(gi[i][e], gi[i][e], q2);
                 }
                 if (pos_row) { acc_l1[0] += a1; acc_s2[0] += q1; acc_l1[2] += a2; acc_s2[2] += q2; }   // UG_u once, IG_i
                 else { acc_l1[4] += a2; acc_s2[4] += q2; }                                               // IG_j
             }
         }
         __syncthreads();
-        {
-            const float pp = (s_pred[0][tr] + s_pred[1][tr]) + (s_pred[2][tr] + s_pred[3][tr]);
-            const float pn = (s_pred[0][tr + kFusedTile] + s_pred[1][tr + kFusedTile]) +
-                             (s_pred[2][tr + kFusedTile] + s_pred[3][tr + kFusedTile]);
+#pragma unroll
+        for (int i = 0; i < 2; ++i) {
+            const int tr = trr[i];
+            const float pp = s_pred[0][tr] + s_pred[1][tr];
+            const float pn = s_pred[0][tr + kFusedTile] + s_pred[1][tr + kFusedTile];
             const float x = pp - pn;                                    // the predict bias cancels in the pair
             const float sg = 1.f / (1.f + expf(-x));
-            if (ok && pos_row && part == 0) acc_loss += -logf(1e-10f + sg);
+            if (ok[i] && pos_row && nh == 0 && quad == 0) acc_loss += -logf(1e-10f + sg);
             const float cbpr = -(sg * (1.f - sg)) / (1e-10f + sg);
-            const float dp = ok ? sign * cbpr : 0.f;                    // d loss / d pred of THIS row
-            float dz[C2];
+            const float dp = ok[i] ? sign * cbpr : 0.f;                 // d loss / d pred of THIS row
+            float dz[4];
 #pragma unroll
-            for (int e = 0; e < C2; ++e) {
-                dz[e] = hval[e] > 0.f ? dp * s_wp[F + part * C2 + e] : 0.f;
+            for (int e = 0; e < 4; ++e) {
+                const int col = nh * 16 + (e >> 1) * 8 + 2 * quad + (e & 1);
+                dz[e] = hval[i][e] > 0.f ? dp * s_wp[F + col] : 0.f;
                 gb2[e] += dz[e];
-                gwh[e] += dp * hval[e];
+                gwh[e] += dp * hval[i][e];
+                gwg[e] += dp * (gu[i][e] * gi[i][e]);
             }
+            image_store2(smem + L::DZ2, L::LBO_T, rbase + 8 * i, nh * 16 + 2 * quad, dz[0], dz[1]);
+            image_store2(smem + L::DZ2, L::LBO_T, rbase + 8 * i, nh * 16 + 8 + 2 * quad, dz[2], dz[3]);
+            if (p.apply && ok[i]) {
 #pragma unroll
-            for (int e = 0; e < CG; ++e) gwg[e] += dp * (gu[e] * gi[e]);
-            image_store8(smem + L::DZ2, L::LBO_T, row, part * C2, dz);
-            if (p.apply && ok) {
-                const int k0 = part * CG;
-#pragma unroll
-                for (int c = 0; c < CG / 4; ++c) {
-                    Vec<4> g1, g2;
-#pragma unroll
-                    for (int e = 0; e < 4; ++e) {
-                        const float w = dp * s_wp[k0 + 4 * c + e];
-                        g1.v[e] = w * gi[4 * c + e];                    // d / d UG[u]
-                        g2.v[e] = w * gu[4 * c + e];                    // d / d IG[item]
-                    }
-                    red_row<4>(p.gUG + (size_t)u * F + k0 + 4 * c, g1);
-                    red_row<4>(p.gIG + (size_t)item * F + k0 + 4 * c, g2);
+                for (int nb = 0; nb < 2; ++nb) {
+                    const int col = nh * 16 + nb * 8 + 2 * quad;
+                    const float w0 = dp * s_wp[col], w1 = dp * s_wp[col + 1];
+                    Vec<2> g1, g2;
+                    g1.v[0] = w0 * gi[i][2 * nb]; g1.v[1] = w1 * gi[i][2 * nb + 1];     // d / d UG[u]
+                    g2.v[0] = w0 * gu[i][2 * nb]; g2.v[1] = w1 * gu[i][2 * nb + 1];     // d / d IG[item]
+                    red_row<2>(p.gUG + (size_t)uu[i] * F + col, g1);
+                    red_row<2>(p.gIG + (size_t)itm[i] * F + col, g2);
                 }
-                if (part == 0) {
+                if (nh == 0 && quad == 0) {
                     if (pos_row) {
-                        red_add_u32(p.cntU + u, 1u);
-                        red_add_u64(p.cntI + item, 1ull);
+                        red_add_u32(p.cntU + uu[i], 1u);
+                        red_add_u64(p.cntI + itm[i], 1ull);
                     } else {
-                        red_add_u64(p.cntI + item, 1ull << 32);
+                        red_add_u64(p.cntI + itm[i], 1ull << 32);
                     }
                 }
             }
         }
-        tc_fence_before();
         asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
         __syncthreads();
         if (!p.apply) {                                      // loss only
@@ -435,150 +373,129 @@ __global__ void __launch_bounds__(kFusedThreads, 1) neumf_fused_kernel(FusedPara
         }
 
         // ---------------------------------------------------------------- dA1 = dZ2 W2 ;  gW2^T += A1^T dZ2
-        if (tid == 0) {
-            tc_fence_after();
-            {   // B = W2 read transposed (MN-major view of its K-major image): mn = in (N1), k = out (N2)
-                const uint32_t id = idesc(N1, false, true);
+        float da1[16];
 #pragma unroll
-                for (int kk = 0; kk < N2 / 16; ++kk)
-                    fused_mma(tmem + L::C_Z1, umma_smem_desc(sbase + L::DZ2 + kk * 2 * L::LBO_T, L::LBO_T, 128),
-                              umma_smem_desc(sbase + L::W2 + kk * 256, 128, L::LBO_W2), id, kk > 0);
-            }
-            {   // A = A1^T (features on the M side, tile rows as K), B = dZ2 read transposed: both MN-major views
-                const uint32_t id = idesc(N2, true, true);
+        for (int e = 0; e < 16; ++e) da1[e] = 0.f;
+        wgmma_fence();
+        // B = W2 read transposed (MN-major view of its K-major image): mn = in (N1), k = out (N2)
 #pragma unroll
-                for (int kk = 0; kk < 128 / 16; ++kk)
-                    fused_mma(tmem + L::C_GW2, umma_smem_desc(sbase + L::A1 + kk * 256, 128, L::LBO_T),
-                              umma_smem_desc(sbase + L::DZ2 + kk * 256, 128, L::LBO_T), id, (!first_tile) || kk > 0);
-            }
-            fused_commit(&s_bar);
-        }
+        for (int kk = 0; kk < N2 / 16; ++kk)
+            wgmma_m64n32<0, 1>(da1, umma_smem_desc(sbase + L::DZ2 + mh * 1024 + kk * 2 * L::LBO_T, L::LBO_T, 128),
+                               umma_smem_desc(sbase + L::W2 + nh * 4 * L::LBO_W2 + kk * 256, 128, L::LBO_W2), kk > 0);
+        // A = A1^T (features on the M side, tile rows of half mh as K), B = dZ2 read transposed: both MN-major views
+#pragma unroll
+        for (int kk = 0; kk < 64 / 16; ++kk)
+            wgmma_m64n16<1, 1>(gw2, umma_smem_desc(sbase + L::A1 + mh * 1024 + kk * 256, 128, L::LBO_T),
+                               umma_smem_desc(sbase + L::DZ2 + nh * 2 * L::LBO_T + mh * 1024 + kk * 256, 128, L::LBO_T), 1u);
+        wgmma_commit();
         if (has_next) prefetch_gmf(next_tile, cur ^ 1);      // the GMF staging has been consumed by the head
-        mbar_wait(&s_bar, phase);
-        phase ^= 1;
-        tc_fence_after();
+        wgmma_wait_all();
+        wgmma_fence_operand(da1);
+        wgmma_fence_operand(gw2);
 
         // ---------------------------------------------------------------- dZ1 = dA1 [A1 > 0] -> image
-        {
-            const int k0 = part * C1;
-            uint32_t r16[16];
-            tmem_ld16_nowait(taddr + (uint32_t)(L::C_Z1 + k0), r16);
-            const uint32_t base = (uint32_t)(row >> 3) * 128u + (uint32_t)(row & 7) * 16u;
-            const uint4 m0 = *reinterpret_cast<const uint4 *>(smem + L::A1 + (uint32_t)(k0 >> 3) * L::LBO_T + base);
-            const uint4 m1 = *reinterpret_cast<const uint4 *>(smem + L::A1 + (uint32_t)((k0 >> 3) + 1) * L::LBO_T + base);
-            const uint32_t mw[8] = {m0.x, m0.y, m0.z, m0.w, m1.x, m1.y, m1.z, m1.w};
-            tmem_wait();
-            float v[16];
 #pragma unroll
-            for (int e = 0; e < 16; ++e) {
-                const uint32_t hbits = (e & 1) ? (mw[e >> 1] >> 16) : (mw[e >> 1] & 0xffffu);   // bf16 of A1[row][k0 + e]
-                const bool on = (hbits & 0x7fffu) != 0u && (hbits & 0x8000u) == 0u;              // > 0
-                v[e] = on ? __uint_as_float(r16[e]) : 0.f;
-                gb1[e] += v[e];
+        for (int nb = 0; nb < 4; ++nb) {
+            const int col = nh * 32 + nb * 8 + 2 * quad;
+#pragma unroll
+            for (int i = 0; i < 2; ++i) {
+                const uint32_t mw = *reinterpret_cast<const uint32_t *>(smem + L::A1 + image_off(L::LBO_T, rbase + 8 * i, col));
+                const float va = bf16_positive(mw & 0xffffu) ? da1[nb * 4 + 2 * i] : 0.f;
+                const float vb = bf16_positive(mw >> 16) ? da1[nb * 4 + 2 * i + 1] : 0.f;
+                gb1[2 * nb] += va;
+                gb1[2 * nb + 1] += vb;
+                image_store2(smem + L::DZ1, L::LBO_T, rbase + 8 * i, col, va, vb);
             }
-            image_store8(smem + L::DZ1, L::LBO_T, row, k0, v);
-            image_store8(smem + L::DZ1, L::LBO_T, row, k0 + 8, v + 8);
         }
-        tc_fence_before();
         asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
         __syncthreads();
 
         // ---------------------------------------------------------------- dA0 = dZ1 W1 ;  gW1^T += A0^T dZ1
-        if (tid == 0) {
-            tc_fence_after();
-            {
-                const uint32_t id = idesc(N0, false, true);
+        float da0[2][16];
 #pragma unroll
-                for (int kk = 0; kk < N1 / 16; ++kk)
-                    fused_mma(tmem + L::C_DA0, umma_smem_desc(sbase + L::DZ1 + kk * 2 * L::LBO_T, L::LBO_T, 128),
-                              umma_smem_desc(sbase + L::W1 + kk * 256, 128, L::LBO_W1), id, kk > 0);
-            }
-            {
-                const uint32_t id = idesc(N1, true, true);
+        for (int s = 0; s < 2; ++s)
 #pragma unroll
-                for (int kk = 0; kk < 128 / 16; ++kk)
-                    fused_mma(tmem + L::C_GW1, umma_smem_desc(sbase + L::A0 + kk * 256, 128, L::LBO_T),
-                              umma_smem_desc(sbase + L::DZ1 + kk * 256, 128, L::LBO_T), id, (!first_tile) || kk > 0);
-            }
-            fused_commit(&s_bar);
+            for (int e = 0; e < 16; ++e) da0[s][e] = 0.f;
+        wgmma_fence();
+#pragma unroll
+        for (int kk = 0; kk < N1 / 16; ++kk) {
+            const uint64_t da = umma_smem_desc(sbase + L::DZ1 + mh * 1024 + kk * 2 * L::LBO_T, L::LBO_T, 128);
+#pragma unroll
+            for (int s = 0; s < 2; ++s)
+                wgmma_m64n32<0, 1>(da0[s], da, umma_smem_desc(sbase + L::W1 + (nh * 8 + s * 4) * L::LBO_W1 + kk * 256, 128, L::LBO_W1),
+                                   kk > 0);
         }
-        mbar_wait(&s_bar, phase);
-        phase ^= 1;
-        tc_fence_after();
+#pragma unroll
+        for (int kk = 0; kk < 128 / 16; ++kk)
+            wgmma_m64n32<1, 1>(gw1, umma_smem_desc(sbase + L::A0 + mh * 8 * L::LBO_T + kk * 256, 128, L::LBO_T),
+                               umma_smem_desc(sbase + L::DZ1 + nh * 4 * L::LBO_T + kk * 256, 128, L::LBO_T), 1u);
+        wgmma_commit();
+        wgmma_wait_all();
+        wgmma_fence_operand(da0[0]);
+        wgmma_fence_operand(da0[1]);
+        wgmma_fence_operand(gw1);
 
-        // ---------------------------------------------------------------- scatter dA0: user half -> gUM[u], item half -> gIM[item]
+        // ---------------------------------------------------------------- scatter dA0: column half 0 -> gUM[u], half 1 -> gIM[item]
+        // lanes 2j and 2j+1 swap half their pairs, so each lane holds 4 consecutive columns of one row: one RED.128 each
         {
-            // parts 0,1: columns [0,64) = the user half of the MLP row; parts 2,3: columns [64,128) = the item half
-            float *dst = (part < 2 ? p.gUM + (size_t)u * D : p.gIM + (size_t)item * D) + (part & 1) * C0;
-            uint32_t ra[16], rb[16];
-            tmem_ld16_nowait(taddr + (uint32_t)(L::C_DA0 + part * C0), ra);
-            tmem_ld16_nowait(taddr + (uint32_t)(L::C_DA0 + part * C0 + 16), rb);
-            tmem_wait();
-            if (ok) {
+            const int odd = lane & 1;
+            float *dst = nh == 0 ? p.gUM + (size_t)uu[odd] * D : p.gIM + (size_t)itm[odd] * D;
 #pragma unroll
-                for (int e4 = 0; e4 < 4; ++e4) {
-                    Vec<4> g;
-                    g.v[0] = __uint_as_float(ra[4 * e4]); g.v[1] = __uint_as_float(ra[4 * e4 + 1]);
-                    g.v[2] = __uint_as_float(ra[4 * e4 + 2]); g.v[3] = __uint_as_float(ra[4 * e4 + 3]);
-                    red_row<4>(dst + 4 * e4, g);
-                }
+            for (int s = 0; s < 2; ++s)
 #pragma unroll
-                for (int e4 = 0; e4 < 4; ++e4) {
+                for (int nb = 0; nb < 4; ++nb) {
+                    const float *d4 = &da0[s][nb * 4];
+                    const float s0 = odd ? d4[0] : d4[2], s1 = odd ? d4[1] : d4[3];
+                    const float r0 = __shfl_xor_sync(0xffffffffu, s0, 1), r1 = __shfl_xor_sync(0xffffffffu, s1, 1);
                     Vec<4> g;
-                    g.v[0] = __uint_as_float(rb[4 * e4]); g.v[1] = __uint_as_float(rb[4 * e4 + 1]);
-                    g.v[2] = __uint_as_float(rb[4 * e4 + 2]); g.v[3] = __uint_as_float(rb[4 * e4 + 3]);
-                    red_row<4>(dst + 16 + 4 * e4, g);
+                    if (odd) { g.v[0] = r0; g.v[1] = r1; g.v[2] = d4[2]; g.v[3] = d4[3]; }
+                    else { g.v[0] = d4[0]; g.v[1] = d4[1]; g.v[2] = r0; g.v[3] = r1; }
+                    if (ok[odd]) red_row<4>(dst + s * 32 + nb * 8 + 2 * (quad & 2), g);
                 }
-            }
         }
         first_tile = false;
-        tc_fence_before();
-        __syncthreads();                                     // A0 / TMEM free for the next tile
+        __syncthreads();                                     // images free for the next tile
     }
 
-    // ---------------------------------------------------------------- once per CTA: weight gradients out of TMEM
-    tc_fence_after();
+    // ---------------------------------------------------------------- once per CTA: weight gradients out of the registers
     if (p.apply && !first_tile) {
         float *gW1 = p.gW, *gb1g = gW1 + (size_t)N1 * N0, *gW2 = gb1g + N1, *gb2g = gW2 + (size_t)N2 * N1, *gwp = gb2g + N2;
-        {   // gW1^T: lane = input feature m (0..N0-1 = 128 rows), column = output n
-            const int n0 = part * C1;
-            uint32_t r16[16];
-            tmem_ld16_nowait(taddr + (uint32_t)(L::C_GW1 + n0), r16);
-            tmem_wait();
 #pragma unroll
-            for (int e = 0; e < 16; ++e) atomicAdd(gW1 + (size_t)(n0 + e) * N0 + row, __uint_as_float(r16[e]));
-        }
-        {   // gW2^T: lanes 0..N1-1 valid
-            const int n0 = part * C2;
-            uint32_t r8[8];
-            tmem_ld8_nowait(taddr + (uint32_t)(L::C_GW2 + n0), r8);       // whole warp executes the collective load
-            tmem_wait();
-            if (row < N1) {
+        for (int nb = 0; nb < 4; ++nb)
 #pragma unroll
-                for (int e = 0; e < 8; ++e) atomicAdd(gW2 + (size_t)(n0 + e) * N1 + row, __uint_as_float(r8[e]));
-            }
-        }
-        // register column sums: warp shuffle over the 32 rows of the warp, then shared, then one global atomic per column
+            for (int i = 0; i < 2; ++i)
 #pragma unroll
-        for (int k = 0; k < C1; ++k) {
+                for (int c = 0; c < 2; ++c)      // gW1^T: row = input feature m, column = output n
+                    atomicAdd(gW1 + (size_t)(nh * 32 + nb * 8 + 2 * quad + c) * N0 + rbase + 8 * i, gw1[nb * 4 + 2 * i + c]);
+#pragma unroll
+        for (int nb = 0; nb < 2; ++nb)
+#pragma unroll
+            for (int i = 0; i < 2; ++i)
+#pragma unroll
+                for (int c = 0; c < 2; ++c)      // gW2^T: rows = the N1 input features (M = 64: no half offset)
+                    atomicAdd(gW2 + (size_t)(nh * 16 + nb * 8 + 2 * quad + c) * N1 + (rbase - mh * 64) + 8 * i, gw2[nb * 4 + 2 * i + c]);
+        // register column sums: shuffle over the 8 row groups of the warp (lanes of equal quad), then shared, then global
+#pragma unroll
+        for (int k = 0; k < 8; ++k) {
             float v = gb1[k];
 #pragma unroll
-            for (int off = 16; off >= 1; off >>= 1) v += __shfl_xor_sync(0xffffffffu, v, off);
-            if (lane == 0) atomicAdd(&s_colsum[part * C1 + k], v);
+            for (int off = 4; off <= 16; off <<= 1) v += __shfl_xor_sync(0xffffffffu, v, off);
+            if (lane < 4) atomicAdd(&s_colsum[nh * 32 + (k >> 1) * 8 + 2 * quad + (k & 1)], v);
         }
 #pragma unroll
-        for (int k = 0; k < C2; ++k) {
+        for (int k = 0; k < 4; ++k) {
             float v = gb2[k], g = gwg[k], h = gwh[k];
 #pragma unroll
-            for (int off = 16; off >= 1; off >>= 1) {
+            for (int off = 4; off <= 16; off <<= 1) {
                 v += __shfl_xor_sync(0xffffffffu, v, off);
                 g += __shfl_xor_sync(0xffffffffu, g, off);
                 h += __shfl_xor_sync(0xffffffffu, h, off);
             }
-            if (lane == 0) {
-                atomicAdd(&s_colsum[N1 + part * C2 + k], v);
-                atomicAdd(&s_colsum[N1 + N2 + part * CG + k], g);
-                atomicAdd(&s_colsum[N1 + N2 + F + part * C2 + k], h);
+            const int col = nh * 16 + (k >> 1) * 8 + 2 * quad + (k & 1);
+            if (lane < 4) {
+                atomicAdd(&s_colsum[N1 + col], v);
+                atomicAdd(&s_colsum[N1 + N2 + col], g);
+                atomicAdd(&s_colsum[N1 + N2 + F + col], h);
             }
         }
         __syncthreads();
@@ -600,9 +517,6 @@ __global__ void __launch_bounds__(kFusedThreads, 1) neumf_fused_kernel(FusedPara
         __syncthreads();
         if (tid < nv && s_red[tid] != 0.0) atomicAdd(p.red + tid, s_red[tid]);
     }
-    tc_fence_before();
-    __syncthreads();
-    if (warp == 0) asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem), "r"(512) : "memory");
 }
 
 template <int F>
@@ -622,8 +536,8 @@ static int launch_neumf_fused_f(const FusedParams &p, cudaStream_t st)
     return DRB_OK;
 }
 
-// The epilogues split every TMEM tile into two column halves of 16-column chunks: factors must be a multiple of 32, and
-// 10 F accumulator columns must fit the 512 of TMEM -> factors = 32 (BASELINE config 3).  Other shapes use the layer-wise path.
+// The warpgroup split of the epilogues is written for factors = 32 (tower 128 -> 64 -> 32, BASELINE config 3); other shapes
+// use the layer-wise path.
 static bool neumf_fused_supported(int F, int L, int mode, float dropout)
 {
     return L == 2 && mode == 0 && dropout == 0.f && F == 32;

@@ -1,4 +1,4 @@
-// nfm.cu -- NFM + BPR on the B200 path (SURVEY 8(f) rank 4).
+// nfm.cu -- NFM + BPR on the GPU path (SURVEY 8(f) rank 4).
 //
 // Stands behind daisy/model/NFMRecommender.py (dropout = 0; the reference's masks come from torch's RNG):
 //   forward   :110-123   e = P[u] * Q[item] -> [BatchNorm1d] -> L x { Linear(F, F) -> [BatchNorm1d] -> relu|sigmoid|tanh }
@@ -654,7 +654,7 @@ extern "C" int drb_nfm_bpr_train_steps_dropout(float *d_P, float *d_Q, float *d_
                 if (rc != DRB_OK) return rc;
                 dz = w.dh;
             }
-            rc = colsum_acc(dz, R, F, gb, st);
+            rc = colsum_pairs_acc(dz, B, F, gb, st);
             if (rc == DRB_OK) rc = gemm_tn_acc_t(tower_dtype, F, F, (int)R, hprev, F, dz, F, gW, F, st);   // gW [out,in] += dz^T h_in
             float *dprev = dz == w.tmp ? w.dh : w.tmp;
             if (rc == DRB_OK) rc = gemm_nn(tower_dtype, R, F, F, dz, F, W, F, dprev, F, st);               // d h_in = dz W

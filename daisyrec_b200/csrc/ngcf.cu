@@ -1,4 +1,4 @@
-// ngcf.cu -- NGCF + BPR on the B200 path (SURVEY 8(f) rank 4).
+// ngcf.cu -- NGCF + BPR on the GPU path (SURVEY 8(f) rank 4).
 //
 // Stands behind daisy/model/NGCFRecommender.py (node_dropout = mess_dropout = 0; the reference's dropout masks come from
 // torch's RNG, and its message dropout is even active at rank() time, :164):

@@ -58,7 +58,7 @@ __device__ __forceinline__ uint32_t mt_temper(uint32_t y)
 //   x[623]   = x[396]   ^ twist(x[623], x[0])                                   -- NEW x[0]: recomputed by its reader
 // every OLD input can be read before anything is written, and every NEW input is a register of the same thread.  So a
 // 624-word block costs: load the old words, ONE barrier, three dependent twists in registers, store + temper + stream the
-// three outputs, ONE barrier -- instead of three load/barrier/store/barrier rounds (58 ms -> see profiles/r02b for 80 M words).
+// three outputs, ONE barrier -- instead of three load/barrier/store/barrier rounds.
 constexpr int kMtThreads = 256;
 
 // regenerate 624-word blocks from the block state in x[] and stream the tempered words to out[0..n): the three-phase walk above

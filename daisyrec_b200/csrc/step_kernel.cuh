@@ -41,6 +41,9 @@ inline int pick_tile(long long per_cta, int cap = kTileDefault)
 #endif
 
 // ------------------------------------------------------------------ device pieces
+// deterministic mode: contribution -> 2^40 fixed point (|sum| < 8.3e6, resolution 9e-13), scalars -> 2^24
+constexpr double kDetScale = 1099511627776.0, kDetAccScale = 16777216.0;
+
 __device__ __forceinline__ float sgnf(float x) { return (float)((x > 0.f) - (x < 0.f)); }
 
 struct Norms {
@@ -111,7 +114,10 @@ __device__ __forceinline__ void apply_row(float *theta_row, float *g_row, float 
 // written for it.  Adam moves every row (dense optimiser semantics of the reference).  Adagrad / RMSprop
 // (AbstractRecommender.py:57-60, torch defaults) keep ONE state row in the m slot: Adagrad leaves an untouched row
 // alone (g = 0 adds nothing), RMSprop's running square of an untouched row still decays by alpha.
-template <int VEC, int W, int NCH, int OPT, bool USERS_ONLY = false>
+// DET (deterministic mode): the gradient is read from the fixed-point sums and assembled with the regulariser in fp64, rounded
+// to fp32 once, and the SGD step rounds lr * g before the subtraction -- the fp64-accumulating oracle's arithmetic, so that the
+// result does not depend on how the compiler contracts the fp32 expression.
+template <int VEC, int W, int NCH, int OPT, bool USERS_ONLY = false, bool DET = false>
 __device__ __forceinline__ void dense_sweep(const StepParams &p, const Norms &nm, const AdamCoef &ac, int gl, int group,
                                             int groups_per_cta, int chunks)
 {
@@ -121,6 +127,7 @@ __device__ __forceinline__ void dense_sweep(const StepParams &p, const Norms &nm
     const int F = p.F;
     for (long long r0 = (long long)blockIdx.x * groups_per_cta + group; r0 < rows; r0 += tg * R) {
         float *th_p[R], *g_p[R], *m_p[R], *v_p[R];
+        long long *g64_p[R];
         unsigned long long cnt[R];
         bool act[R], is_user[R];
         Row<VEC, W, NCH> th[R], g[R], m[R], v[R];
@@ -133,6 +140,7 @@ __device__ __forceinline__ void dense_sweep(const StepParams &p, const Norms &nm
             size_t o = (size_t)(act[k] ? it : 0) * F;
             th_p[k] = (is_user[k] ? p.P : p.Q) + o;
             g_p[k] = (is_user[k] ? p.ws.gP : p.ws.gQ) + o;
+            if constexpr (DET) g64_p[k] = (is_user[k] ? p.ws.gP64 : p.ws.gQ64) + o;
             cnt[k] = 0;
             if (act[k]) cnt[k] = is_user[k] ? (unsigned long long)__ldcg(p.ws.cntU + it) : __ldcg(p.ws.cntI + it);
             th[k] = load_row<VEC, W, NCH>(th_p[k], gl, chunks, act[k]);
@@ -159,13 +167,27 @@ __device__ __forceinline__ void dense_sweep(const StepParams &p, const Norms &nm
                 Vec<VEC> &t = th[k].c[ch];
 #pragma unroll
                 for (int e = 0; e < VEC; ++e) {
-                    float x = t.v[e], gg = p.gscale * g[k].c[ch].v[e];
-                    if (touched) {
-                        float sg = p.reg1 * sgnf(x);
-                        gg += ca * (sg + p.reg2 * x * ia) + cb * (sg + p.reg2 * x * ib);
+                    float x = t.v[e], gg;
+                    if constexpr (DET) {
+                        long long *fx_p = g64_p[k] + c * VEC + e;
+                        const long long fx = __ldcg(fx_p);
+                        double gd = (double)p.gscale * ((double)fx / kDetScale);
+                        if (touched) {
+                            const double sg = (double)(p.reg1 * sgnf(x));
+                            gd += (double)ca * (sg + (double)__fmul_rn(__fmul_rn(p.reg2, x), ia)) +
+                                  (double)cb * (sg + (double)__fmul_rn(__fmul_rn(p.reg2, x), ib));
+                        }
+                        if (fx != 0) __stcg(fx_p, 0ll);
+                        gg = (float)gd;
+                    } else {
+                        gg = p.gscale * g[k].c[ch].v[e];
+                        if (touched) {
+                            float sg = p.reg1 * sgnf(x);
+                            gg += ca * (sg + p.reg2 * x * ia) + cb * (sg + p.reg2 * x * ib);
+                        }
                     }
                     if constexpr (OPT == DRB_OPT_SGD) {
-                        t.v[e] = x - p.lr * gg;
+                        t.v[e] = DET ? __fsub_rn(x, __fmul_rn(p.lr, gg)) : x - p.lr * gg;
                     } else if constexpr (OPT == DRB_OPT_ADAGRAD) {   // sum += g^2; theta -= lr g / (sqrt(sum) + 1e-10)
                         float ss = m[k].c[ch].v[e] + gg * gg;
                         t.v[e] = x - p.lr * (gg / (sqrtf(ss) + 1e-10f));
@@ -223,8 +245,6 @@ __device__ __forceinline__ int draw_negative(const StepParams &p, int u, unsigne
 template <bool LEAN> struct RowOffset { typedef size_t type; };
 template <> struct RowOffset<true> { typedef unsigned type; };
 
-// deterministic mode: contribution -> 2^40 fixed point (|sum| < 8.3e6, resolution 9e-13), scalars -> 2^24
-constexpr double kDetScale = 1099511627776.0, kDetAccScale = 16777216.0;
 __device__ __forceinline__ void det_red(long long *p, float v)
 {
     red_add_u64(reinterpret_cast<unsigned long long *>(p), (unsigned long long)__double2ll_rn((double)v * kDetScale));
@@ -397,7 +417,10 @@ __device__ __forceinline__ void bpr_steps_body(StepParams &p, XCH &xch)
                         return s1 + s2;
                     }
                     const float x = pos - neg;
-                    const float sg = 1.f / (1.f + expf(-x));
+                    // deterministic mode: exp in fp64, rounded once -- the correctly rounded expf of the host's libm, so the
+                    // coefficient (it scales every contribution of the triple) is the fp64 oracle's to the bit
+                    const float ex = (GEN && p.det) ? (float)exp(-(double)x) : expf(-x);
+                    const float sg = 1.f / (1.f + ex);
                     c_pos = -(sg * (1.f - sg)) / (1e-10f + sg);
                     c_neg = -c_pos;
                     return -logf(1e-10f + sg);
@@ -525,17 +548,8 @@ __device__ __forceinline__ void bpr_steps_body(StepParams &p, XCH &xch)
         if (p.phases == 3) grid_barrier(&hdr->barrier, epoch);
         if (!(p.phases & 2)) break;   // split mode: the host reduces gQ / counters / acc across ranks now
         if (GEN && p.det) {
-            // fixed-point sums -> the fp32 accumulators phase 2 reads (one rounding per element, whatever order the atomics took)
-            const long long gsz = (long long)gridDim.x * kThreads, gt = (long long)blockIdx.x * kThreads + tid;
-            const long long nP = (long long)p.U * F, nQ = (long long)p.I * F;
-            for (long long k = gt; k < nP + nQ; k += gsz) {
-                long long *src = k < nP ? p.ws.gP64 + k : p.ws.gQ64 + (k - nP);
-                const long long v = __ldcg(src);
-                if (v != 0) {
-                    __stcg((k < nP ? p.ws.gP + k : p.ws.gQ + (k - nP)), (float)((double)v / kDetScale));
-                    __stcg(src, 0ll);
-                }
-            }
+            // fixed-point scalar sums -> acc (the table sums stay in fixed point: the DET sweep reads and clears them)
+            const long long gt = (long long)blockIdx.x * kThreads + tid;
             if (gt < 8) {
                 acc[gt] = (double)__ldcg(p.ws.accfx + gt) / kDetAccScale;
                 __stcg(p.ws.accfx + gt, 0ll);
@@ -583,14 +597,25 @@ __device__ __forceinline__ void bpr_steps_body(StepParams &p, XCH &xch)
                 ac.step_size = (float)((double)p.lr / (1.0 - pow((double)p.beta1, t)));
                 ac.bc2_sqrt = (float)sqrt(1.0 - pow((double)p.beta2, t));
             }
-            const bool dense = p.dense_hint >= 0 ? (p.dense_hint != 0)
-                                                 : ((p.opt != DRB_OPT_SGD) || (3 * nb >= ((long long)p.U + p.I) / 4));
+            const bool dense = (GEN && p.det) || (p.dense_hint >= 0 ? (p.dense_hint != 0)
+                                                                 : ((p.opt != DRB_OPT_SGD) || (3 * nb >= ((long long)p.U + p.I) / 4)));
             if constexpr (XCH::kActive) {
                 // this rank's item slice: reduce the ranks' accumulators, update, broadcast the new rows; then the local user
                 // rows are swept below with the item half switched off (p.I = 0 inside the policy's copy of the parameters)
                 xch.template item_slice<VEC, W, NCH>(p, s, nm, ac, gl, group, GROUPS, chunks, epoch);
             }
-            if (dense || p.opt != DRB_OPT_SGD) {   // stateful optimisers always sweep (claim mode is SGD only)
+            if (GEN && p.det) {                    // single GPU only (launch_steps): no exchange policy is active here
+                if constexpr (GEN && !XCH::kActive) {
+                    if (p.opt == DRB_OPT_SGD)
+                        dense_sweep<VEC, W, NCH, DRB_OPT_SGD, false, true>(p, nm, ac, gl, group, GROUPS, chunks);
+                    else if (p.opt == DRB_OPT_ADAM)
+                        dense_sweep<VEC, W, NCH, DRB_OPT_ADAM, false, true>(p, nm, ac, gl, group, GROUPS, chunks);
+                    else if (p.opt == DRB_OPT_ADAGRAD)
+                        dense_sweep<VEC, W, NCH, DRB_OPT_ADAGRAD, false, true>(p, nm, ac, gl, group, GROUPS, chunks);
+                    else
+                        dense_sweep<VEC, W, NCH, DRB_OPT_RMSPROP, false, true>(p, nm, ac, gl, group, GROUPS, chunks);
+                }
+            } else if (dense || p.opt != DRB_OPT_SGD) {   // stateful optimisers always sweep (claim mode is SGD only)
                 if (p.opt == DRB_OPT_SGD)
                     dense_sweep<VEC, W, NCH, DRB_OPT_SGD, XCH::kActive>(p, nm, ac, gl, group, GROUPS, chunks);
                 else if (p.opt == DRB_OPT_ADAM)

@@ -1,21 +1,19 @@
-// umma_gemm.cuh -- bf16 tensor-core GEMM for the NeuMF tower on sm_100a: tcgen05.mma with the accumulator in TMEM.
+// umma_gemm.cuh -- bf16 tensor-core GEMM for the NeuMF tower on sm_90a: wgmma with fp32 accumulators in registers.
 //
 //   C[M,N] (op)= opA(A)[M,K] * opB(B)[K,N]       A, B, C fp32 in global memory; operands are rounded to bf16
-//   while they are staged into shared memory, products accumulate in fp32 in tensor memory.
+//   while they are staged into shared memory, products accumulate in fp32 in the registers of the issuing warpgroup.
 //
 // Same call signature and epilogues as the fp32 CUDA-core sgemm_kernel in neumf.cu, so the three GEMM call sites of
 // the tower (forward NT + bias + ReLU, input-gradient NN + ReLU mask, weight-gradient TN split-K) switch by dtype.
 //
-// One CTA (128 threads) owns a 128-row tile of C and the full N (<= 256):
-//   * TMEM: `cols` columns (power of two >= 32) x 128 lanes hold the fp32 accumulator (tcgen05.alloc by warp 0);
-//   * per 32-deep K chunk all threads stage A[128x32] and B[Npad x 32] into shared memory in the canonical
+// One CTA (two warpgroups, 256 threads) owns a 128-row tile of C and NT >= N columns (NT in {32, 64, 128, 256}):
+//   * per 32-deep K chunk all threads stage A[128x32] and B[NT x 32] into shared memory in the canonical
 //     no-swizzle core-matrix layouts (8 x 16-byte core matrices; K-major for operands that are contiguous along K,
 //     MN-major for the transposed operands of the backward GEMMs; LBO / SBO padded so the 16-byte staging stores are
-//     bank-conflict free), fence.proxy.async, then ONE thread issues two tcgen05.mma (K = 16 each, M = 128,
-//     N = Npad) and tcgen05.commit's an mbarrier that releases the buffers;
-//   * epilogue: warp w reads TMEM lanes [32w, 32w+32) with tcgen05.ld.32x32b.x32 (lane == output row), transposes the
-//     32x32 block through shared memory and writes row-contiguous fp32 with bias / ReLU / mask fused, or atomically
-//     accumulates (optionally transposed) for the split-K weight gradient.
+//     bank-conflict free), fence.proxy.async, then warpgroup g issues wgmma.m64n32k16 over rows [64g, 64g + 64) for
+//     every 32-column slice of B and waits for its own group;
+//   * epilogue: each thread owns two rows x NT/4 columns of the accumulator fragment and writes them with bias / ReLU /
+//     mask fused, or atomically accumulates (optionally transposed) for the split-K weight gradient.
 // The tower GEMMs are skinny (N, K <= 128 against M ~ 10^6): they are bound by streaming A from HBM, not by the
 // tensor pipe, so the kernel relies on several resident CTAs per SM for overlap rather than on an intra-CTA pipeline.
 #pragma once
@@ -27,28 +25,61 @@ namespace drb {
 
 constexpr int kUmmaBK = 32;        // K elements staged per chunk (2 MMAs of K=16)
 constexpr int kUmmaMaxN = 256;
+constexpr int kUmmaThreads = 256;  // two warpgroups, 64 tile rows each
 
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
-
+// wgmma shared-memory matrix descriptor, no swizzle: start [0,14) >>4, LBO [16,30) >>4, SBO [32,46) >>4,
+// base_offset [49,52) = 0, layout_type [62,64) = 0 (interleave).  LBO is the stride between core matrices along K,
+// SBO the stride between core matrices along M / N, for K-major and MN-major operands alike.
 __device__ __forceinline__ uint64_t umma_smem_desc(uint32_t smem_addr, uint32_t lbo_bytes, uint32_t sbo_bytes)
 {
-    // cute::UMMA::SmemDescriptor: start [0,14) >>4, LBO [16,30) >>4, SBO [32,46) >>4, version [46,48) = 1,
-    // base_offset [49,52) = 0, lbo_mode [52] = 0, layout_type [61,64) = 0 (SWIZZLE_NONE / interleave)
     uint64_t d = 0;
     d |= (uint64_t)((smem_addr >> 4) & 0x3fffu);
     d |= (uint64_t)((lbo_bytes >> 4) & 0x3fffu) << 16;
     d |= (uint64_t)((sbo_bytes >> 4) & 0x3fffu) << 32;
-    d |= (uint64_t)1 << 46;
     return d;
 }
 
-__device__ __forceinline__ uint32_t umma_idesc_bf16_f32(int M, int N, bool a_mn = false, bool b_mn = false)
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_wait_all() { asm volatile("wgmma.wait_group.sync.aligned 0;" ::: "memory"); }
+
+// keeps the compiler from moving accesses of an accumulator across the asynchronous MMA that owns it
+template <int N>
+__device__ __forceinline__ void wgmma_fence_operand(float (&d)[N])
 {
-    // cute::UMMA::InstrDescriptor: c_format [4,6) = 1 (F32), a_format [7,10) = 1 (BF16), b_format [10,13) = 1 (BF16),
-    // a_major [15] = 0, b_major [16] = 0 (K-major), n_dim [17,23) = N >> 3, m_dim [24,29) = M >> 4
-    return (1u << 4) | (1u << 7) | (1u << 10) | ((a_mn ? 1u : 0u) << 15) | ((b_mn ? 1u : 0u) << 16) |
-           ((uint32_t)(N >> 3) << 17) | ((uint32_t)(M >> 4) << 24);
+#pragma unroll
+    for (int e = 0; e < N; ++e) asm volatile("" : "+f"(d[e])::"memory");
+}
+
+// D[64 x 32] (+)= A[64 x 16] * B[16 x 32], bf16 operands from shared memory, fp32 accumulators.  TA / TB: 0 = K-major,
+// 1 = MN-major operand image.  Fragment: d[4 nb + 2 i + c] = D(16 warp + lane / 4 + 8 i, 8 nb + 2 (lane % 4) + c).
+template <int TA, int TB>
+__device__ __forceinline__ void wgmma_m64n32(float (&d)[16], uint64_t da, uint64_t db, uint32_t accumulate)
+{
+    asm volatile(
+        "{\n\t"
+        ".reg .pred p;\n\t"
+        "setp.ne.b32 p, %18, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n32k16.f32.bf16.bf16 "
+        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, %16, %17, p, 1, 1, %19, %20;\n\t"
+        "}\n"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]),
+          "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15])
+        : "l"(da), "l"(db), "r"(accumulate), "n"(TA), "n"(TB));
+}
+// the same with 16 columns: d[4 nb + 2 i + c], nb in {0, 1}
+template <int TA, int TB>
+__device__ __forceinline__ void wgmma_m64n16(float (&d)[8], uint64_t da, uint64_t db, uint32_t accumulate)
+{
+    asm volatile(
+        "{\n\t"
+        ".reg .pred p;\n\t"
+        "setp.ne.b32 p, %10, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n16k16.f32.bf16.bf16 "
+        "{%0, %1, %2, %3, %4, %5, %6, %7}, %8, %9, p, 1, 1, %11, %12;\n\t"
+        "}\n"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7])
+        : "l"(da), "l"(db), "r"(accumulate), "n"(TA), "n"(TB));
 }
 
 __device__ __forceinline__ uint32_t pack_bf16x2(float a, float b)
@@ -114,125 +145,85 @@ __device__ __forceinline__ void umma_stage_tile(unsigned char *smem, int rows, c
 
 // EPI 0: C = acc   1: C = relu(acc + bias[n])   2: C = acc * (ref(m,n) > 0)   3: atomicAdd(C, acc) (split-K over grid.z)
 // EPI 4: atomicAdd(C^T, acc) -- transposed accumulate C[n*ldc + m] (split-K)
-template <bool TA, bool TB, int EPI>
-__global__ void __launch_bounds__(128) umma_gemm_kernel(int M, int N, int K, const float *__restrict__ A, long long lda,
-                                                        const float *__restrict__ B, long long ldb, float *__restrict__ C,
-                                                        long long ldc, const float *__restrict__ bias,
-                                                        const float *__restrict__ ref, long long ldref, int k_chunk, int Npad,
-                                                        int tmem_cols, float alpha)
+template <bool TA, bool TB, int EPI, int NT>
+__global__ void __launch_bounds__(kUmmaThreads) umma_gemm_kernel(int M, int N, int K, const float *__restrict__ A, long long lda,
+                                                                 const float *__restrict__ B, long long ldb, float *__restrict__ C,
+                                                                 long long ldc, const float *__restrict__ bias,
+                                                                 const float *__restrict__ ref, long long ldref, int k_chunk,
+                                                                 float alpha)
 {
     constexpr int kABytes = (kUmmaBK / 8) * (128 / 8) * 144;                 // worst case (MN-major) A tile
-    constexpr int kBBytes = (kUmmaBK / 8) * (kUmmaMaxN / 8) * 144;
-    __shared__ __align__(128) unsigned char s_all[kABytes + kBBytes];         // A tile | B tile; reused by the epilogue
+    constexpr int kBBytes = (kUmmaBK / 8) * (NT / 8) * 144;
+    constexpr int NS = NT / 32;                                               // 32-column slices per warpgroup
+    __shared__ __align__(128) unsigned char s_all[kABytes + kBBytes];
     unsigned char *sA = s_all, *sB = s_all + kABytes;
     // A(m,k) = A[k*lda + m] (TA) and B(k,n) = B[k*ldb + n] (!TB) are contiguous along the MN dimension -> MN-major tiles
     constexpr bool A_MN = TA, B_MN = !TB;
-    __shared__ __align__(8) uint64_t s_bar;
-    __shared__ uint32_t s_tmem;
-    const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
+    const int tid = threadIdx.x, wg = tid >> 7, warp = (tid >> 5) & 3, lane = tid & 31;
     const long long m0 = (long long)blockIdx.x * 128;
     const int kb = (EPI >= 3) ? blockIdx.z * k_chunk : 0;
     const int ke = (EPI >= 3) ? min(K, kb + k_chunk) : K;
 
-    if (warp == 0) {
-        asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(&s_tmem)), "r"(tmem_cols)
-                     : "memory");
-        asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-    }
-    if (tid == 0) {
-        mbar_init(&s_bar, 1);
-        fence_mbar_init();
-    }
-    tc_fence_before();
-    __syncthreads();
-    tc_fence_after();
-    const uint32_t tmem = s_tmem;
-    const uint32_t idesc = umma_idesc_bf16_f32(128, Npad, A_MN, B_MN);
-    const uint32_t lboA = umma_lbo(A_MN, 128), lboB = umma_lbo(B_MN, Npad);
-    uint32_t phase = 0;
-    bool first = true;
+    float acc[NS][16];
+#pragma unroll
+    for (int s = 0; s < NS; ++s)
+#pragma unroll
+        for (int e = 0; e < 16; ++e) acc[s][e] = 0.f;
+    const uint32_t lboA = umma_lbo(A_MN, 128), lboB = umma_lbo(B_MN, NT);
+    const uint32_t sboA = umma_sbo(A_MN), sboB = umma_sbo(B_MN);
+    const uint32_t aBase = smem_u32(sA) + (uint32_t)wg * 8u * sboA, bBase = smem_u32(sB);   // this warpgroup's 64 rows
     for (int k0 = kb; k0 < ke; k0 += kUmmaBK) {
-        umma_stage_tile<A_MN>(sA, 128, A, lda, m0, M, k0, ke, tid, 128);
-        umma_stage_tile<B_MN>(sB, Npad, B, ldb, 0, N, k0, ke, tid, 128);
+        umma_stage_tile<A_MN>(sA, 128, A, lda, m0, M, k0, ke, tid, kUmmaThreads);
+        umma_stage_tile<B_MN>(sB, NT, B, ldb, 0, N, k0, ke, tid, kUmmaThreads);
         asm volatile("fence.proxy.async.shared::cta;" ::: "memory");   // generic-proxy stores -> visible to the tensor core
         __syncthreads();
-        if (tid == 0) {
-            tc_fence_after();
+        wgmma_fence();
 #pragma unroll
-            for (int kk = 0; kk < kUmmaBK / 16; ++kk) {
-                uint64_t da = umma_smem_desc(smem_u32(sA) + kk * 2 * lboA, lboA, umma_sbo(A_MN));
-                uint64_t db = umma_smem_desc(smem_u32(sB) + kk * 2 * lboB, lboB, umma_sbo(B_MN));
-                uint32_t acc = (first && kk == 0) ? 0u : 1u;
-                asm volatile(
-                    "{\n\t"
-                    ".reg .pred p;\n\t"
-                    "setp.ne.b32 p, %4, 0;\n\t"
-                    "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t"
-                    "}\n" ::"r"(tmem),
-                    "l"(da), "l"(db), "r"(idesc), "r"(acc)
-                    : "memory");
-            }
-            // commit: arrives on the mbarrier once every MMA issued so far has finished reading smem / writing TMEM
-            asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(smem_u32(&s_bar))
-                         : "memory");
+        for (int kk = 0; kk < kUmmaBK / 16; ++kk) {
+            const uint64_t da = umma_smem_desc(aBase + kk * 2 * lboA, lboA, sboA);
+#pragma unroll
+            for (int s = 0; s < NS; ++s)
+                wgmma_m64n32<A_MN, B_MN>(acc[s], da, umma_smem_desc(bBase + s * 4 * sboB + kk * 2 * lboB, lboB, sboB), 1u);
         }
-        first = false;
-        mbar_wait(&s_bar, phase);
-        phase ^= 1;
-        tc_fence_after();
+        wgmma_commit();
+        wgmma_wait_all();
+#pragma unroll
+        for (int s = 0; s < NS; ++s) wgmma_fence_operand(acc[s]);
+        __syncthreads();                                                 // both warpgroups done reading before restaging
     }
-    // epilogue: lane == output row inside this warp's 32-lane quarter of TMEM.  32 columns at a time are pulled out with
-    // one tcgen05.ld.32x32b.x32, transposed through a padded shared-memory tile (the operand buffers are free now) and
-    // written / accumulated with row-contiguous, fully coalesced accesses (lane == column).
-    float *tile = reinterpret_cast<float *>(s_all) + warp * (32 * 33);
-    const long long mrow0 = m0 + warp * 32;
-    const uint32_t taddr = tmem + ((uint32_t)(warp * 32) << 16);
-    const bool any = kb < ke;
-    for (int c = 0; c < Npad; c += 32) {
-        uint32_t r[32];
-        if (c + 32 <= Npad) {
-            asm volatile(
-                "tcgen05.ld.sync.aligned.32x32b.x32.b32 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-                "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-                : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]),
-                  "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]), "=r"(r[16]),
-                  "=r"(r[17]), "=r"(r[18]), "=r"(r[19]), "=r"(r[20]), "=r"(r[21]), "=r"(r[22]), "=r"(r[23]), "=r"(r[24]),
-                  "=r"(r[25]), "=r"(r[26]), "=r"(r[27]), "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-                : "r"(taddr + (uint32_t)c));
-        } else {   // Npad is a multiple of 16: a trailing half chunk
-            asm volatile(
-                "tcgen05.ld.sync.aligned.32x32b.x16.b32 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, [%16];"
-                : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]),
-                  "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15])
-                : "r"(taddr + (uint32_t)c));
+    if (kb >= ke) return;
+    const long long mrow = m0 + wg * 64 + warp * 16 + (lane >> 2);
 #pragma unroll
-            for (int e = 16; e < 32; ++e) r[e] = 0u;
-        }
-        asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
+    for (int s = 0; s < NS; ++s) {
 #pragma unroll
-        for (int e = 0; e < 32; ++e) tile[lane * 33 + e] = __uint_as_float(r[e]);
-        __syncwarp();
-        const int n = c + lane;
-        if (any && n < N) {
-            const float bn = (EPI == 1) ? bias[n] : 0.f;
-            for (int rr = 0; rr < 32; ++rr) {
-                const long long m = mrow0 + rr;
-                if (m >= M) break;
-                float v = tile[rr * 33 + lane];
-                if (EPI == 1) { v += bn; v = v > 0.f ? v : 0.f; }
-                if (EPI == 2) { v = (ref[m * ldref + n] > 0.f) ? v * alpha : 0.f; }
-                if (EPI == 3) atomicAdd(C + m * ldc + n, v);
-                else if (EPI == 4) atomicAdd(C + (long long)n * ldc + m, v);
-                else C[m * ldc + n] = v;
+        for (int nb = 0; nb < 4; ++nb) {
+#pragma unroll
+            for (int i = 0; i < 2; ++i) {
+                const long long m = mrow + 8 * i;
+                if (m >= M) continue;
+#pragma unroll
+                for (int c = 0; c < 2; ++c) {
+                    const int n = s * 32 + nb * 8 + 2 * (lane & 3) + c;
+                    if (n >= N) continue;
+                    float v = acc[s][nb * 4 + i * 2 + c];
+                    if (EPI == 1) { v += bias[n]; v = v > 0.f ? v : 0.f; }
+                    if (EPI == 2) { v = (ref[m * ldref + n] > 0.f) ? v * alpha : 0.f; }
+                    if (EPI == 3) atomicAdd(C + m * ldc + n, v);
+                    else if (EPI == 4) atomicAdd(C + (long long)n * ldc + m, v);
+                    else C[m * ldc + n] = v;
+                }
             }
         }
-        __syncwarp();
     }
-    tc_fence_before();
-    __syncthreads();
-    if (warp == 0) {
-        asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem), "r"(tmem_cols) : "memory");
-    }
+}
+
+template <bool TA, bool TB, int EPI, int NT>
+static void launch_umma_gemm_nt(dim3 grid, long long M, int N, int K, const float *A, long long lda, const float *B, long long ldb,
+                                float *C, long long ldc, const float *bias, const float *ref, long long ldref, int k_chunk,
+                                cudaStream_t st, float alpha)
+{
+    umma_gemm_kernel<TA, TB, EPI, NT><<<grid, kUmmaThreads, 0, st>>>((int)M, N, K, A, lda, B, ldb, C, ldc, bias, ref, ldref,
+                                                                     k_chunk, alpha);
 }
 
 template <bool TA, bool TB, int EPI>
@@ -242,9 +233,6 @@ static int launch_umma_gemm(long long M, int N, int K, const float *A, long long
 {
     if (M <= 0 || N <= 0 || K <= 0) return DRB_OK;
     DRB_REQUIRE(N <= kUmmaMaxN, "umma_gemm: N=%d exceeds %d", N, kUmmaMaxN);
-    int Npad = (N + 15) / 16 * 16;
-    int cols = 32;
-    while (cols < Npad) cols <<= 1;
     dim3 grid((unsigned)((M + 127) / 128), 1, 1);
     int k_chunk = K;
     if (EPI >= 3) {   // split-K: the [out x in] result is one tile, parallelism comes from the K (row) dimension.
@@ -257,8 +245,10 @@ static int launch_umma_gemm(long long M, int N, int K, const float *A, long long
         k_chunk = (int)(((K + chunks - 1) / chunks + kUmmaBK - 1) / kUmmaBK * kUmmaBK);
         grid.z = (unsigned)((K + k_chunk - 1) / k_chunk);
     }
-    umma_gemm_kernel<TA, TB, EPI><<<grid, 128, 0, st>>>((int)M, N, K, A, lda, B, ldb, C, ldc, bias, ref, ldref, k_chunk, Npad, cols,
-                                                        alpha);
+    if (N <= 32) launch_umma_gemm_nt<TA, TB, EPI, 32>(grid, M, N, K, A, lda, B, ldb, C, ldc, bias, ref, ldref, k_chunk, st, alpha);
+    else if (N <= 64) launch_umma_gemm_nt<TA, TB, EPI, 64>(grid, M, N, K, A, lda, B, ldb, C, ldc, bias, ref, ldref, k_chunk, st, alpha);
+    else if (N <= 128) launch_umma_gemm_nt<TA, TB, EPI, 128>(grid, M, N, K, A, lda, B, ldb, C, ldc, bias, ref, ldref, k_chunk, st, alpha);
+    else launch_umma_gemm_nt<TA, TB, EPI, 256>(grid, M, N, K, A, lda, B, ldb, C, ldc, bias, ref, ldref, k_chunk, st, alpha);
     DRB_CUDA(cudaGetLastError());
     return DRB_OK;
 }

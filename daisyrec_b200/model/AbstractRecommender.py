@@ -1,4 +1,4 @@
-"""Host side of the B200 recommenders: the reference's plug-in surface
+"""Host side of the GPU-path recommenders: the reference's plug-in surface
 (daisy/model/AbstractRecommender.py:10-137) without nn.Module / autograd / torch.optim.
 
 ``GeneralRecommender.fit(train_loader)`` keeps the reference contract -- a
@@ -146,7 +146,7 @@ class AbstractRecommender(object):
         if name == 'sparse_adam':       # what optim.SparseAdam.step() raises on nn.Embedding's dense gradients (:61-62)
             raise RuntimeError('SparseAdam does not support dense gradients, please consider Adam instead')
         if name in ('adagrad', 'rmsprop'):
-            raise NotImplementedError(f"optimizer '{name}' is outside the B200 hot path of {type(self).__name__} "
+            raise NotImplementedError(f"optimizer '{name}' is outside the GPU hot path of {type(self).__name__} "
                                       f"(native: {', '.join(self.SUPPORTED_OPTIMIZERS)})")
         if self.logger is not None:
             self.logger.info('Received unrecognized optimizer, set default Adam optimizer')
@@ -159,7 +159,7 @@ class AbstractRecommender(object):
         if lt in self.SUPPORTED_LOSSES:
             return
         if lt in ('CL', 'SL', 'HL', 'TL', 'BPR'):
-            raise NotImplementedError(f"loss_type '{lt}' is outside the B200 hot path of {type(self).__name__} "
+            raise NotImplementedError(f"loss_type '{lt}' is outside the GPU hot path of {type(self).__name__} "
                                       f"(native: {', '.join(self.SUPPORTED_LOSSES)})")
         raise NotImplementedError(f'Invalid loss type: {self.loss_type}...')
 

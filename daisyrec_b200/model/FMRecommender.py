@@ -1,4 +1,4 @@
-"""FM on the B200 path, with the reference's class name, config keys and methods
+"""FM on the GPU path, with the reference's class name, config keys and methods
 (daisy/model/FMRecommender.py:16-131).
 
 FM here is MF's factor product plus first-order terms: ``pred = <p_u, q_i> + (u_bias[u] + i_bias[i]) + bias_``

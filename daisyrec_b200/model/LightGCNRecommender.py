@@ -1,4 +1,4 @@
-"""LightGCN + BPR on the B200 path, with the reference's class name, config keys and methods
+"""LightGCN + BPR on the GPU path, with the reference's class name, config keys and methods
 (daisy/model/LightGCNRecommender.py:23-211).
 
 The ego table E0 = cat(embed_user.weight, embed_item.weight) is one contiguous device tensor
@@ -47,7 +47,7 @@ class LightGCN(GeneralRecommender):
         self.restore_item_e = None
 
         m = self.interaction_matrix
-        # optional B200 key 'adj_builder': 'host' (default; numpy restatement of get_norm_adj_mat, values bit-identical to
+        # optional GPU-path key 'adj_builder': 'host' (default; numpy restatement of get_norm_adj_mat, values bit-identical to
         # scipy's) | 'device' (sorted CSR + transpose + D^-1/2 A D^-1/2 built by csr.cu; 1/sqrt instead of pow: fp32
         # values equal except on rare rounding ties)
         if str(config.get('adj_builder', 'host')) == 'device':

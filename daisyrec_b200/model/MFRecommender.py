@@ -1,4 +1,4 @@
-"""BPR-MF on the B200 path, with the reference's class name, config keys and methods
+"""BPR-MF on the GPU path, with the reference's class name, config keys and methods
 (daisy/model/MFRecommender.py:25-133).
 
 No nn.Embedding, no autograd, no torch.optim: the two factor tables are raw fp32 device tensors
@@ -60,14 +60,14 @@ class MF(GeneralRecommender):
         self._opt_steps = 0
         self._stage = None
         self.step_variant = ops.mf_step_variant(self.factors, self.user_num + self.item_num)   # runs the one-off on-device selection
-        # optional B200 key: True = every cross-thread sum of a step in fixed point (bitwise reproducible runs); single GPU
+        # optional GPU-path key: True = every cross-thread sum of a step in fixed point (bitwise reproducible runs); single GPU
         self.deterministic = bool(config.get('deterministic', False))
         if self.deterministic and (self.world > 1 or str(config.get('neg_sampling', 'table')) == 'fused'):
             raise NotImplementedError("deterministic=True covers single-GPU training on the sampler's triples")
-        # optional B200 key (torchrun only): 'p2p' = one persistent launch per epoch with the exchange inside the kernel over
+        # optional GPU-path key (torchrun only): 'p2p' = one persistent launch per epoch with the exchange inside the kernel over
         # peer-mapped memory; 'nccl' = phase 1 -> grouped NCCL all-reduce -> phase 2 per step (also the automatic fallback)
         self.sharded_comm = str(config.get('sharded_comm', 'auto'))   # auto: p2p on 2 GPUs, nccl beyond (parallel.py)
-        # optional B200 key: 'table' (default; the reference's per-user-once negatives, taken from the loader's triples) |
+        # optional GPU-path key: 'table' (default; the reference's per-user-once negatives, taken from the loader's triples) |
         # 'fused' (throughput mode: a fresh negative per triple and step is drawn inside the step kernel from the
         # complement of the user's train row; the loader's third column is ignored)
         self.neg_sampling = str(config.get('neg_sampling', 'table'))
@@ -296,7 +296,7 @@ class MF(GeneralRecommender):
         return ops.mf_full_rank(self._full_user_table(), self.embed_item.weight, users, k)[0].cpu().numpy()
 
     def full_rank_users(self, users):
-        """Batched full_rank (B200 extension): int64 ndarray [len(users), topk]."""
+        """Batched full_rank (GPU extension): int64 ndarray [len(users), topk]."""
         users = torch.as_tensor(np.asarray(users, dtype=np.int64)).to(self.device)
         k = min(self.topk, self.item_num)
         return ops.mf_full_rank(self._full_user_table(), self.embed_item.weight, users, k).cpu().numpy()

@@ -1,4 +1,4 @@
-"""NFM + BPR on the B200 path, with the reference's class name, config keys and methods
+"""NFM + BPR on the GPU path, with the reference's class name, config keys and methods
 (daisy/model/NFMRecommender.py:14-209).
 
 Factor tables ``embed_user.weight`` / ``embed_item.weight``, the first-order terms in one packed vector (``u_bias.weight``,

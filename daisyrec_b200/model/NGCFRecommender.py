@@ -1,4 +1,4 @@
-"""NGCF + BPR on the B200 path, with the reference's class name, config keys and methods
+"""NGCF + BPR on the GPU path, with the reference's class name, config keys and methods
 (daisy/model/NGCFRecommender.py:61-252; node_dropout = 0).
 
 The ego table E0 = cat(embed_user.weight, embed_item.weight) is one contiguous device tensor; the BiGNN layers live in
@@ -39,7 +39,7 @@ class NGCF(GeneralRecommender):
         self.node_dropout = config['node_dropout']
         self.message_dropout = config['mess_dropout']
         if float(self.node_dropout or 0.0) != 0.0:
-            raise NotImplementedError('NGCF on the B200 path runs with node_dropout = 0 (the reference default; a sparse dropout '
+            raise NotImplementedError('NGCF on the GPU path runs with node_dropout = 0 (the reference default; a sparse dropout '
                                       'of the adjacency drawn from the torch RNG)')
         self.message_dropout = float(self.message_dropout or 0.0)
         if not 0.0 <= self.message_dropout < 1.0:
@@ -52,7 +52,7 @@ class NGCF(GeneralRecommender):
         self.early_stop = config['early_stop']
         dims = self.hidden_size_list
         if any(int(d) < 1 or int(d) > 256 for d in dims):
-            raise NotImplementedError('NGCF on the B200 path supports layer widths up to 256')
+            raise NotImplementedError('NGCF on the GPU path supports layer widths up to 256')
 
         # reference RNG stream (:95-116): two nn.Embedding constructors, per BiGNN layer two nn.Linear constructors, then
         # apply(_init_weight) over embed_user, embed_item and every (linear, interact_transform) pair

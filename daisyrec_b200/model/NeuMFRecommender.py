@@ -1,4 +1,4 @@
-"""NeuMF + BPR on the B200 path, with the reference's class name, config keys and methods
+"""NeuMF + BPR on the GPU path, with the reference's class name, config keys and methods
 (daisy/model/NeuMFRecommender.py:15-232; model_name 'NeuMF', 'GMF', 'MLP' and 'NeuMF-pre').
 
 Four raw fp32 embedding tables (``embed_user_GMF/embed_item_GMF/embed_user_MLP/embed_item_MLP`` ``.weight``)
@@ -41,7 +41,7 @@ class NeuMF(GeneralRecommender):
         if not (0.0 <= self.dropout < 1.0):
             raise ValueError(f'dropout must be in [0, 1), got {self.dropout}')
         if self.factors % 4 != 0:
-            raise NotImplementedError('NeuMF on the B200 path needs factors to be a multiple of 4 (128-bit rows)')
+            raise NotImplementedError('NeuMF on the GPU path needs factors to be a multiple of 4 (128-bit rows)')
         F, Ln = self.factors, self.num_layers
         D = F * (2 ** (Ln - 1))
         self.mlp_dim = D
@@ -80,14 +80,14 @@ class NeuMF(GeneralRecommender):
         self._ws = None
         self._opt_steps = 0
         self._rows = int(config.get('neumf_scratch_rows', 1 << 16))
-        # optional B200 key: 'fp32' (CUDA cores, parity path, default) | 'bf16' (tcgen05 tensor cores, BASELINE config 3)
-        #                   | 'fused' (bf16 tcgen05, the whole tower step of a 64-triple tile inside one CTA: activations stay in
-        #                     shared / tensor memory; factors = 32, num_layers = 2, dropout 0 -- other shapes run as 'bf16')
+        # optional GPU-path key: 'fp32' (CUDA cores, parity path, default) | 'bf16' (wgmma tensor cores, BASELINE config 3)
+        #                   | 'fused' (bf16 wgmma, the whole tower step of a 64-triple tile inside one CTA: activations stay in
+        #                     shared memory, accumulators in registers; factors = 32, num_layers = 2, dropout 0 -- other shapes run as 'bf16')
         td = str(config.get('tower_dtype', 'fp32')).lower()
         if td not in ('fp32', 'bf16', 'fused'):
             raise ValueError(f"tower_dtype must be 'fp32', 'bf16' or 'fused', got {td!r}")
         self._tower_dtype = {'fp32': 0, 'bf16': 1, 'fused': 2}[td]
-        # optional B200 key: how nn.Dropout's masks (:61) are produced in train mode.
+        # optional GPU-path key: how nn.Dropout's masks (:61) are produced in train mode.
         #   'torch'  : torch itself draws them on the host, in the reference's order (per step: the pos forward's L masks, then
         #              the neg forward's), from the global CPU generator; they are bit-packed and uploaded -- the reference's
         #              masks bit for bit.  Costs one host bernoulli_ per layer and forward: meant for small batches.
@@ -111,7 +111,7 @@ class NeuMF(GeneralRecommender):
             return torch.as_tensor(t).detach().to('cpu', torch.float32)
 
         def tower_parts(model):
-            """(per-layer (weight, bias) list, predict weight [1, k], predict bias [1]) of a B200 NeuMF or an nn.Module one."""
+            """(per-layer (weight, bias) list, predict weight [1, k], predict bias [1]) of a GPU-path NeuMF or an nn.Module one."""
             if hasattr(model, 'tower'):
                 flat, F, Ln = cpu(model.tower), model.factors, model.num_layers
                 out, o = [], 0

@@ -27,7 +27,7 @@ def _dev(t, dtype, name):
 
 def require_cuda():
     if not torch.cuda.is_available():
-        raise RuntimeError("daisyrec_b200 needs a CUDA device (sm_100a); there is no CPU fallback")
+        raise RuntimeError("daisyrec_b200 needs a CUDA device (sm_90a); there is no CPU fallback")
 
 
 def hyper(lr, reg_1, reg_2, opt="sgd", beta1=0.9, beta2=0.999, eps=1e-8, loss="BPR"):

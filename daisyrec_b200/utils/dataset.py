@@ -2,7 +2,7 @@
 
 ``BasicDataset`` and ``CandidatesDataset`` stay ordinary ``torch.utils.data.Dataset`` objects so
 that drivers written for daisyRec (run_examples/test.py:93-94,118-119) work unchanged; the
-B200 models do not iterate them sample by sample -- ``fit``/``rank`` read ``.data`` in bulk.
+GPU-path models do not iterate them sample by sample -- ``fit``/``rank`` read ``.data`` in bulk.
 """
 import torch
 from torch.utils.data import DataLoader, Dataset

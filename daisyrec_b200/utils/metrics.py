@@ -11,7 +11,7 @@ Reference quirks kept: duplicate ids in a rank list each count as a hit (np.in1d
 1 for that reason; NDCG's ideal DCG uses the number of hits INSIDE the list (:230), not |gt|;
 'f1' / 'auc' cannot be reached through Metric.run (:87-90 compare the previous KPI, not the name) and
 raise ValueError here too; 'map' runs in Metric.run but has no display name, so calc_ranking_results
-raises KeyError on it exactly like :38.  'diversity' (item categories) is outside the B200 path.
+raises KeyError on it exactly like :38.  'diversity' (item categories) is outside the GPU path.
 """
 import os
 
@@ -70,7 +70,7 @@ def _kpi_table(test_ur, pred_ur, test_u, ks, item_num, item_pop):
 def _check_names(names):
     for mc in names:
         if mc == 'diversity':
-            raise NotImplementedError("'diversity' needs config['i_categories']; it is outside the B200 evaluation path")
+            raise NotImplementedError("'diversity' needs config['i_categories']; it is outside the GPU evaluation path")
         if mc not in _DEVICE_KPIS:
             raise ValueError(f'Invalid metric name {mc}')          # metrics.py:91-92 (also where 'f1' / 'auc' end up)
 

@@ -76,7 +76,7 @@ class BasicNegtiveSampler(AbstractSampler):
         self.sample_method = config['sample_method']
         self.sample_ratio = config['sample_ratio']
         self.loss_type = config['loss_type'].upper()
-        # optional B200 keys (absent == reference behaviour)
+        # optional GPU-path key (absent == reference behaviour)
         self.rng_engine = config.get('sampler_rng', 'numpy')       # 'numpy' (MT19937 replay) | 'philox'
         self.csr = config.get('train_csr', None)                   # (row_ptr int64, col int32) to skip the dict walk
 

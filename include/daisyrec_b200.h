@@ -1,5 +1,5 @@
 /*
- * daisyrec_b200.h -- C ABI of the B200-native BPR hot path (libdaisyrec_b200.so).
+ * daisyrec_b200.h -- C ABI of the H100-native (sm_90a) BPR hot path (libdaisyrec_b200.so).
  *
  * The reference (AmazingDD/daisyRec v2.3.0) is pure Python: it has no FFI, so the
  * "boundary" it offers is the duck-typed model / sampler contract consumed by
@@ -36,7 +36,7 @@ extern "C" {
 #define DRB_ERR_CUDA 2        /* a CUDA runtime call failed; see drb_last_error()                 */
 #define DRB_ERR_NAN_LOSS 3    /* loss became NaN: ValueError of AbstractRecommender.py:122-123    */
 #define DRB_ERR_EMPTY_SET 4   /* a user has no un-interacted item: numpy "a cannot be empty"      */
-#define DRB_ERR_NO_DEVICE 5   /* no sm_100 device / kernel image not loadable on this device     */
+#define DRB_ERR_NO_DEVICE 5   /* no sm_90 device / kernel image not loadable on this device     */
 #define DRB_ERR_PEER 6        /* multi-GPU peer exchange: a rank did not reach the rendezvous in time */
 
 #define DRB_OPT_SGD 0         /* optim.SGD(lr)   AbstractRecommender.py:55-56                     */
@@ -248,7 +248,7 @@ int drb_fm_predict(const float *d_P, const float *d_Q, const float *d_bias, int3
  * drb_ngcf_forward_dropout / drb_ngcf_bpr_train_steps_dropout  the same with nn.Dropout(mess_dropout) of :164 active (reference
  *    default 0.1; the reference builds the module inside forward(), so it drops at rank() time too): d_keep = the masks torch
  *    draws, one per layer over its [(U+I), width] output, as bytes, layers concatenated (train_steps: steps concatenated).
- * Layer widths: 1..256.  tower_dtype as for NeuMF (0 fp32, 1 bf16 tcgen05 GEMMs). */
+ * Layer widths: 1..256.  tower_dtype as for NeuMF (0 fp32, 1 bf16 wgmma GEMMs). */
 int64_t drb_ngcf_param_count(const int32_t *h_dims, int32_t num_layers);
 size_t drb_ngcf_workspace_bytes(int32_t user_num, int32_t item_num, const int32_t *h_dims, int32_t num_layers, int32_t opt);
 int drb_ngcf_workspace_init(void *d_ws, int32_t user_num, int32_t item_num, const int32_t *h_dims, int32_t num_layers,
@@ -388,8 +388,8 @@ int drb_neumf_scores(const float *d_UG, const float *d_IG, const float *d_UM, co
                      void *d_ws, int32_t user_num, int32_t item_num, int32_t factors, int32_t num_layers, int32_t opt,
                      int64_t max_rows, const int64_t *d_users, int64_t n_users, const int64_t *d_items, int32_t per_user,
                      int32_t tower_dtype, int32_t mode, float *d_scores, void *stream);
-/* tower_dtype: 0 = fp32 on CUDA cores (parity path), 1 = bf16 operands on tcgen05 tensor cores with the fp32
- * accumulator in tensor memory (BASELINE config 3).  drb_gemm_test exposes the tower's GEMM dispatcher to the tests:
+/* tower_dtype: 0 = fp32 on CUDA cores (parity path), 1 = bf16 operands on wgmma tensor cores with the fp32
+ * accumulators in registers (BASELINE config 3).  drb_gemm_test exposes the tower's GEMM dispatcher to the tests:
  * variant 0 NT+bias+ReLU (forward), 1 NN+ReLU-mask (input gradient), 2 NN, 3 TN split-K accumulate (weight gradient). */
 int drb_gemm_test(int32_t variant, int32_t dtype, int64_t M, int32_t N, int32_t K, const float *d_A, int64_t lda,
                   const float *d_B, int64_t ldb, float *d_C, int64_t ldc, const float *d_bias, const float *d_ref,

@@ -1,6 +1,6 @@
 """Time the REFERENCE's own host-side producers / consumers of the hot path on this machine's CPU (build container only:
 imports /root/reference through oracle/ref_harness.py).  TEST INFRASTRUCTURE -- gives the CPU side of the section-8(f)
-rows whose GPU side is in profiles/r01i_eval_bench.json.  Shapes are cut down where the reference is O(U * I) in Python and
+rows whose GPU side is bench.py's configs.inference / sampling / shuffle lines.  Shapes are cut down where the reference is O(U * I) in Python and
 the full-size time is extrapolated linearly in the number of users (stated in the output).
 
     python -m oracle.time_reference_producers

@@ -93,7 +93,7 @@ def main():
             n_in //= 2
         flop_triple = 2 * 3 * flop                          # 2 items x (fwd + 2 bwd GEMMs)
         print(json.dumps(dict(model="NeuMF", shape="ml-20m", F=F, L=L, batch=B, ms_per_step=ms, triples_per_s=B / ms * 1e3,
-                              tower_TFLOPs=B * flop_triple / ms / 1e9, tower="fp32 CUDA cores" if a.tower == "fp32" else "bf16 tcgen05 (TMEM accumulator)")))
+                              tower_TFLOPs=B * flop_triple / ms / 1e9, tower="fp32 CUDA cores" if a.tower == "fp32" else "bf16 wgmma (register accumulators)")))
     elif a.what == "mf-fused":
         # throughput mode: negatives drawn inside the step kernel (Philox + k-th complement over the CSR row)
         U, I, nnz = SHAPES["ml-20m"]

@@ -7,12 +7,12 @@ python daisyrec_b200/_build.py >/dev/null
 mkdir -p daisyrec_b200/lib/variants
 for cfg in "$@"; do
   mb=${cfg%%_*}; un=${cfg##*_}
-  nvcc -gencode arch=compute_100a,code=sm_100a -O3 -std=c++17 -lineinfo -Xcompiler -fPIC -DDRB_MINB=$mb -DDRB_UNR=$un \
+  nvcc -gencode arch=compute_90a,code=sm_90a -O3 -std=c++17 -lineinfo -Xcompiler -fPIC -DDRB_MINB=$mb -DDRB_UNR=$un \
        -c daisyrec_b200/csrc/mf_bpr.cu -o daisyrec_b200/lib/variants/mf_bpr_${cfg}.o &
 done
 wait
 for cfg in "$@"; do
-  nvcc -gencode arch=compute_100a,code=sm_100a -shared -cudart static -o daisyrec_b200/lib/variants/lib_${cfg}.so \
+  nvcc -gencode arch=compute_90a,code=sm_90a -shared -cudart static -o daisyrec_b200/lib/variants/lib_${cfg}.so \
        daisyrec_b200/lib/variants/mf_bpr_${cfg}.o $(ls daisyrec_b200/lib/*.o | grep -v '/mf_bpr.o$') -ldl
   rm daisyrec_b200/lib/variants/mf_bpr_${cfg}.o
 done

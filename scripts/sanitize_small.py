@@ -43,7 +43,7 @@ E0 = t((rng.standard_normal((U + I, F)) * .1).astype(np.float32))
 lws = ops.LgcnWorkspace(U, I, F, "adam", dev)
 ops.lgcn_propagate(E0, lws, graph, 2)
 ops.lgcn_bpr_train_steps(E0, lws, graph, 2, bu, bi, bj, B, 0, 2, ops.hyper(0.01, 0.001, 0.001, "adam"))
-# NeuMF fp32 + bf16 (tcgen05) + dropout
+# NeuMF fp32 + bf16 (wgmma) + dropout
 Fn, L = 32, 2; D = Fn * 2
 tabs = [t((rng.standard_normal(s) * .2).astype(np.float32)) for s in ((U, Fn), (I, Fn), (U, D), (I, D))]
 W = t((rng.standard_normal(ops.neumf_param_count(Fn, L)) * .1).astype(np.float32))

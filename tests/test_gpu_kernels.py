@@ -1,4 +1,4 @@
-"""GPU parity tests (run with -m gpu on the B200 box): the CUDA path, called through the C ABI
+"""GPU parity tests (run with -m gpu on an H100): the CUDA path, called through the C ABI
 (daisyrec_b200.ops -> libdaisyrec_b200.so), against the golden fixtures of the real reference and
 against the CPU oracle on seeded random inputs.
 

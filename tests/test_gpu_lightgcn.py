@@ -81,7 +81,7 @@ def test_lightgcn_vs_oracle_random(ops, orc, F, L, opt, reg):
 
 
 def test_lightgcn_dropin_class(ops, orc):
-    """The reference's call sequence (test.py:88-95,118-120) on the B200 LightGCN class."""
+    """The reference's call sequence (test.py:88-95,118-120) on the GPU-path LightGCN class."""
     from daisyrec_b200.model.LightGCNRecommender import LightGCN
     from daisyrec_b200.utils.dataset import BasicDataset, CandidatesDataset, get_dataloader
     g = golden("lightgcn")

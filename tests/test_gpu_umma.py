@@ -1,4 +1,4 @@
-"""tcgen05 (bf16 operands, fp32 TMEM accumulator) GEMM of the NeuMF tower vs a float64 product of the bf16-rounded
+"""wgmma (bf16 operands, fp32 register accumulators) GEMM of the NeuMF tower vs a float64 product of the bf16-rounded
 operands, and the bf16-tower training step vs the fp32 tower (BASELINE config 3 tolerance)."""
 import numpy as np
 import pytest
@@ -75,7 +75,7 @@ def test_umma_weight_gradient_transposed_accumulate(ops, Mi, No, R):
 
 
 def test_neumf_bf16_tower_step_close_to_fp32(ops):
-    """One NeuMF step with the tcgen05 bf16 tower vs the fp32 tower: loss within 2e-3 relative, tables within bf16 noise."""
+    """One NeuMF step with the wgmma bf16 tower vs the fp32 tower: loss within 2e-3 relative, tables within bf16 noise."""
     rng = np.random.default_rng(0)
     U, I, F, L, B = 500, 400, 32, 2, 4096
     D = F * 2 ** (L - 1)
@@ -104,9 +104,9 @@ def test_neumf_bf16_tower_step_close_to_fp32(ops):
 @pytest.mark.parametrize("B,reg", [(64, 0.0), (4096, 0.001), (5000, 0.002), (130, 0.001)])
 def test_neumf_fused_tower_matches_layerwise_bf16(ops, B, reg):
     """tower_dtype 2 (the whole tower step of a 64-triple tile fused in one CTA: bf16 operand images in shared memory, every
-    accumulator in TMEM, transposed operands read through swapped-stride descriptors) against tower_dtype 1 (the same bf16
+    accumulator in registers, transposed operands read through swapped-stride descriptors) against tower_dtype 1 (the same bf16
     products as separate GEMM launches).  Both round the same values to bf16 at the same points, so they agree to fp32
-    accumulation-order noise: a wrong descriptor, TMEM column or image offset shows up as an O(1) error in exactly one of
+    accumulation-order noise: a wrong descriptor, fragment column or image offset shows up as an O(1) error in exactly one of
     {loss (forward), embedding tables (dZ W products), tower block (A^T dZ products, bias / predict sums)}."""
     rng = np.random.default_rng(B)
     U, I, F, L = 700, 500, 32, 2
@@ -140,7 +140,7 @@ def test_neumf_fused_tower_matches_layerwise_bf16(ops, B, reg):
 
 
 def test_neumf_fused_tower_multi_step_training(ops):
-    """Several chained Adam steps over many tiles per CTA (TMEM weight-gradient accumulators carried across tiles, flushed once)."""
+    """Several chained Adam steps over many tiles per CTA (register weight-gradient accumulators carried across tiles, flushed once)."""
     rng = np.random.default_rng(9)
     U, I, F, L, B, K = 3000, 2000, 32, 2, 20000, 3
     D = F * 2 ** (L - 1)

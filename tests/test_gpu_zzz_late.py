@@ -206,7 +206,7 @@ def test_ngcf_class_runs_the_reference_default_config():
 def test_neumf_fused_tower_kpi_impact_is_small():
     """NeuMF (F = 32, tower 128 -> 64 -> 32, Adam, dropout 0) trained for two epochs on the ML-100K fixture triples (the config-1
     data: 943 x 1 152, 313 452 triples, batch 256) from the same initial weights and the same batch order, once with the fp32
-    tower and once with the fused bf16 tcgen05 tower: NDCG@10 / HR@10 on the fixture's 304 test users x 1 000 candidates move by
+    tower and once with the fused bf16 wgmma tower: NDCG@10 / HR@10 on the fixture's 304 test users x 1 000 candidates move by
     less than the stated bound (bf16 rounds every product operand to 8 bits of mantissa; the gap is training noise, not bias)."""
     from daisyrec_b200 import ops
     from daisyrec_b200.model import NeuMF

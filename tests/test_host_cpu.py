@@ -261,20 +261,20 @@ def test_epoch_seed_and_permutation_follow_the_dataloader():
 
 
 def test_reference_arm_times_the_installed_reference(tmp_path):
-    """bench.py --impl reference runs the REAL daisy MF.fit (oracle/_ref) over its own DataLoader; config is the own arm's."""
+    """bench.py --impl reference runs the REAL daisy MF.fit (oracle/_ref) over its own DataLoader when build() installed it,
+    else the PyTorch-CPU port (oracle/torch_port.py), and says which; config is the own arm's."""
     import json
     import subprocess
     import sys
     from conftest import ROOT
     sys.path.insert(0, ROOT)
     import bench
-    if bench.reference_root() is None:
-        pytest.skip("oracle/_ref not installed (no /root/reference in this container)")
+    kind = "port" if bench.reference_root() is None else "reference"
     r = subprocess.run([sys.executable, os.path.join(ROOT, "bench.py"), "--impl", "reference", "--shape", "tiny", "--batch",
                         "2048", "--steps", "3", "--warmup", "1", "--quick"], capture_output=True, text=True, timeout=600)
     assert r.returncode == 0, r.stderr[-2000:]
     line = json.loads(r.stdout.strip().splitlines()[-1])
-    assert line["impl"] == "reference" and line["cpu_baseline"]["kind"] == "reference" and line["value"] > 0
+    assert line["impl"] == "reference" and line["cpu_baseline"]["kind"] == kind and line["value"] > 0
     assert line["steps"] == 3 and line["gpu_launches"] == 0
     ns = type("A", (), dict(shape="tiny", num_ng=4, factors=64, batch=2048))
     assert line["config"] == bench.workload_config(ns, 1)                  # same_config with the own arm
@@ -351,3 +351,36 @@ def test_mt19937_jump_table_matches_numpy():
     s0 = np.random.RandomState(5).get_state()[1].copy()
     for m in (3, 6):
         assert same(jump(polys[m + 1], s0), jump(polys[m], jump(polys[m], s0))), m
+
+
+def test_bench_dump_outputs_is_seeded_and_bounded(tmp_path):
+    """bench.py --dump-outputs: small arrays are written whole; an array above its share of the 64 MB budget becomes the same
+    seeded sample of its rows on every run (or of its elements when one row alone exceeds the share); the files stay within
+    the budget and keep float32 / float64."""
+    import subprocess
+    import sys
+    sys.path.insert(0, ROOT)
+    import bench
+    rng = np.random.default_rng(3)
+    arrays = {"big_rows": rng.standard_normal((120_000, 64)).astype(np.float32),           # 30.7 MB > 64 MB / 3
+              "one_wide_row": rng.standard_normal((1, 6_000_000)).astype(np.float32),      # 24 MB in a single row
+              "loss": np.array([1.25], np.float64)}
+    outs = []
+    for run in range(2):
+        d = tmp_path / f"run{run}"
+        bench.dump_outputs(str(d), arrays)
+        outs.append({n: np.load(d / (n + ".npy")) for n in arrays})
+        total = sum(os.path.getsize(d / (n + ".npy")) for n in arrays)
+        assert total <= bench.DUMP_BYTES, total
+    a, b = outs
+    for n in arrays:
+        assert a[n].dtype == arrays[n].dtype and np.array_equal(a[n], b[n]), n
+    assert np.array_equal(a["loss"], arrays["loss"])
+    share = bench.DUMP_BYTES // 3
+    assert a["big_rows"].shape == (share // 256, 64)
+    rows = {r.tobytes() for r in arrays["big_rows"]}
+    assert all(r.tobytes() in rows for r in a["big_rows"][:50])                          # whole rows of the original
+    assert a["one_wide_row"].size == share // 4 and np.isin(a["one_wide_row"][:100], arrays["one_wide_row"]).all()
+    r = subprocess.run([sys.executable, os.path.join(ROOT, "bench.py"), "--impl", "reference", "--dump-outputs",
+                        str(tmp_path / "x")], capture_output=True, text=True, timeout=120)
+    assert r.returncode != 0 and "--dump-outputs" in r.stderr
