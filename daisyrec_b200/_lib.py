@@ -245,6 +245,16 @@ class DrbError(RuntimeError):
         self.code = code
 
 
+# the errors the reference raises for these conditions (AbstractRecommender.py:122-123; numpy's choice() on an empty population)
+NAN_LOSS_MESSAGE = "Loss=Nan or Infinity: current settings does not fit the recommender"
+EMPTY_SET_MESSAGE = "'a' cannot be empty unless no samples are taken"
+
+
 def check(rc):
-    if rc != DRB_OK:
-        raise DrbError(rc, (lib().drb_last_error() or b"").decode(errors="replace"))
+    if rc == DRB_OK:
+        return
+    if rc == DRB_ERR_NAN_LOSS:
+        raise ValueError(NAN_LOSS_MESSAGE)
+    if rc == DRB_ERR_EMPTY_SET:
+        raise ValueError(EMPTY_SET_MESSAGE)
+    raise DrbError(rc, (lib().drb_last_error() or b"").decode(errors="replace"))

@@ -79,14 +79,13 @@ extern "C" int drb_index_range_check(const void *d_ids, int32_t elem_bytes, int6
     long long h_buf[8] = {0, 0, 0, 0, 0, 0, 0, 0};
     for (int c = 0; c < n_cols; ++c) h_buf[c] = h_hi[c];
     DRB_CUDA(cudaMemcpyAsync(d_buf, h_buf, sizeof(h_buf), cudaMemcpyHostToDevice, st));
-    long long blocks = (n_rows * n_cols + 1023) / 1024, cap = (long long)sm_count() * 8;
-    if (blocks > cap) blocks = cap;
+    const int blocks = grid_for(n_rows * n_cols, 1024, 8);
     if (elem_bytes == 4)
-        index_range_kernel<int32_t><<<(int)blocks, 256, 0, st>>>((const int32_t *)d_ids, n_rows, n_cols, d_buf,
-                                                                 (unsigned long long *)(d_buf + 4));
+        index_range_kernel<int32_t><<<blocks, 256, 0, st>>>((const int32_t *)d_ids, n_rows, n_cols, d_buf,
+                                                            (unsigned long long *)(d_buf + 4));
     else
-        index_range_kernel<int64_t><<<(int)blocks, 256, 0, st>>>((const int64_t *)d_ids, n_rows, n_cols, d_buf,
-                                                                 (unsigned long long *)(d_buf + 4));
+        index_range_kernel<int64_t><<<blocks, 256, 0, st>>>((const int64_t *)d_ids, n_rows, n_cols, d_buf,
+                                                            (unsigned long long *)(d_buf + 4));
     DRB_CUDA(cudaGetLastError());
     DRB_CUDA(cudaMemcpyAsync(h_buf, d_buf, sizeof(h_buf), cudaMemcpyDeviceToHost, st));
     DRB_CUDA(cudaStreamSynchronize(st));

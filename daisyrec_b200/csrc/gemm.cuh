@@ -1,8 +1,11 @@
-// gemm.cuh -- plain entry points of the dense-layer GEMM dispatcher in neumf.cu (dtype 0: fp32 CUDA cores, 1: bf16 wgmma).
+// gemm.cuh -- plain entry points of the dense-layer helpers in neumf.cu: the GEMM dispatcher (dtype 0: fp32 CUDA cores,
+// 1: bf16 wgmma), bias-gradient column sums and the optimiser step on a flat parameter block.
 #pragma once
 #include "common.cuh"
 
 namespace drb {
+
+struct WsHeader;
 
 // C[M,N] = A[M,K] B[N,K]^T        (Linear forward: activations x weight^T)
 int gemm_nt(int dtype, long long M, int N, int K, const float *A, long long lda, const float *B, long long ldb, float *C,
@@ -17,5 +20,9 @@ int gemm_tn_acc_t(int dtype, long long M, int N, int K, const float *A, long lon
 int colsum_acc(const float *dZ, long long M, int N, float *gb, cudaStream_t st);
 // the same over the 2B rows of a pairwise step, each pos row m added to its neg row B + m first
 int colsum_pairs_acc(const float *dZ, long long B, int N, float *gb, cudaStream_t st);
+// optimiser step of h on the flat block W[n] with gradient g (SGD, or torch.optim.Adam's single-tensor rule with state m, v at
+// step adam_step0 + 1); clears g.  Does nothing once hdr->status is set (a NaN loss).
+int dense_update(float *W, float *g, float *m, float *v, long long n, const drb_hyper *h, long long adam_step0,
+                 const WsHeader *hdr, cudaStream_t st);
 
 }  // namespace drb

@@ -167,10 +167,8 @@ int launch_spmm(const Adj &a, const float *X, float *Y, float *S, int F, cudaStr
     DRB_REQUIRE(k != nullptr, "unsupported factors=%d", F);
     DRB_CUDA(cudaMemsetAsync(Y, 0, sizeof(float) * (size_t)a.n * F, st));   // zero-degree rows + RED targets
     if (a.nseg == 0) return DRB_OK;
-    long long groups = (kSpmmThreads / 32) * (32 / g.width);
-    long long blocks = (a.nseg + groups - 1) / groups, cap = (long long)sm_count() * 8;
-    if (blocks > cap) blocks = cap;
-    k<<<(int)blocks, kSpmmThreads, 0, st>>>(a, X, Y, S, F);
+    const int groups = (kSpmmThreads / 32) * (32 / g.width);
+    k<<<grid_for(a.nseg, groups, 8), kSpmmThreads, 0, st>>>(a, X, Y, S, F);
     DRB_CUDA(cudaGetLastError());
     return DRB_OK;
 }
@@ -192,10 +190,7 @@ static int propagate_sum(const Adj &a, const float *X0, float *S, float *Xa, flo
 static int scale_table(float *x, long long n, float s, cudaStream_t st)
 {
     long long n4 = n / 4;
-    if (n4 > 0) {
-        long long blocks = (n4 + 255) / 256, cap = (long long)sm_count() * 16;
-        scale_kernel<<<(int)(blocks > cap ? cap : blocks), 256, 0, st>>>(x, n4, s);
-    }
+    if (n4 > 0) scale_kernel<<<grid_for(n4, 256), 256, 0, st>>>(x, n4, s);
     if (n4 * 4 < n) scale_tail_kernel<<<1, 32, 0, st>>>(x, n4 * 4, n, s);
     DRB_CUDA(cudaGetLastError());
     return DRB_OK;
@@ -293,21 +288,16 @@ extern "C" int drb_lgcn_bpr_train_steps(float *d_E0, void *d_ws, int32_t U, int3
         if (rc == DRB_OK) rc = scale_table(w.Em, nn * F, inv, st);
         if (rc != DRB_OK) return rc;
         // phase 1 on the propagated tables (scores) + ego tables (norms): G = dL/dE_mean
-        StepParams p;
+        StepParams p = one_step(h, U, I, F, d_bu + base, d_bi + base, d_bj + base, nb, adam_step0 + s);
+        p.loss = DRB_LOSS_BPR;                                   // BPR only: the loss id of h is not read
         p.P = w.Em; p.Q = w.Em + (size_t)U * F;
         p.ws.hdr = w.hdr; p.ws.gP = w.G; p.ws.gQ = w.G + (size_t)U * F; p.ws.cntU = w.cntU; p.ws.cntI = w.cntI;
         p.ws.mP = w.m; p.ws.vP = w.v; p.ws.mQ = w.m ? w.m + (size_t)U * F : nullptr; p.ws.vQ = w.v ? w.v + (size_t)U * F : nullptr;
-        p.bu = d_bu + base; p.bi = d_bi + base; p.bj = d_bj + base;
-        p.n = nb; p.batch = nb; p.first_step = 0; p.n_steps = 1;
-        p.U = U; p.I = I; p.F = F; p.tile = 512;
-        p.lr = h->lr; p.reg1 = h->reg_1; p.reg2 = h->reg_2; p.opt = h->opt;
-        p.beta1 = h->beta1; p.beta2 = h->beta2; p.eps = h->eps; p.adam_step0 = adam_step0 + s;
         p.step_loss = d_step_loss + s;
         p.apply = apply ? 1 : 0;
         p.dense_hint = 1;
         p.Pn = d_E0; p.Qn = d_E0 + (size_t)U * F;
-        p.gscale = 1.f; p.dense_grad = 1; p.neg_mult = 1.f; p.keep_counts = 0;
-        p.neg_row_ptr = nullptr; p.neg_col = nullptr; p.neg_out = nullptr; p.neg_seed = 0ull; p.loss = DRB_LOSS_BPR;
+        p.dense_grad = 1;
         if (!apply) {
             p.phases = 3;                                        // loss only: both phases in one launch, no update
             return launch_steps(p, st, /*keep_status=*/true);

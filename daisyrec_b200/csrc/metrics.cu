@@ -191,13 +191,6 @@ __global__ void kpi_finish_kernel(KpiParams p, int grid, double *out)
     }
 }
 
-static int kpi_grid(long long n)
-{
-    long long g = (n + KPI_WARPS - 1) / KPI_WARPS, cap = (long long)sm_count() * 4;
-    if (g > cap) g = cap;
-    return (int)(g < 1 ? 1 : g);
-}
-
 static long long kpi_words(int item_num) { return ((long long)item_num + 31) / 32; }
 
 }  // namespace drb
@@ -235,7 +228,7 @@ extern "C" int drb_rank_metrics(const float *d_preds, int64_t n_users, int32_t l
     p.bitmap = (uint32_t *)d_ws;
     p.partial = (double *)((char *)d_ws + bitmap_bytes);
     DRB_CUDA(cudaMemsetAsync(p.bitmap, 0, bitmap_bytes, st));
-    const int grid = kpi_grid(n_users);
+    const int grid = grid_for(n_users, KPI_WARPS, 4);   // 4 per SM: the workspace holds sm_count() * 4 partial rows
     kpi_kernel<<<grid, KPI_WARPS * 32, 0, st>>>(p);
     DRB_CUDA(cudaGetLastError());
     kpi_finish_kernel<<<1, 256, 0, st>>>(p, grid, d_out);

@@ -252,10 +252,8 @@ static int launch_predict(const float *d_P, const float *d_Q, int32_t F, const i
     PredictKernel k = g.vec == 4 ? pick_predict_v<4>(g.width, g.nch)
                                  : g.vec == 2 ? pick_predict_v<2>(g.width, g.nch) : pick_predict_v<1>(g.width, g.nch);
     DRB_REQUIRE(k != nullptr, "unsupported factors=%d", F);
-    long long per_block = (256 / 32) * (32 / g.width);
-    long long blocks = (n + per_block - 1) / per_block, cap = (long long)sm_count() * 8;
-    if (blocks > cap) blocks = cap;
-    k<<<(int)blocks, 256, 0, (cudaStream_t)stream>>>(d_P, d_Q, F, d_u, d_i, n, d_out, d_bias, U, I);
+    const int per_block = (256 / 32) * (32 / g.width);
+    k<<<grid_for(n, per_block, 8), 256, 0, (cudaStream_t)stream>>>(d_P, d_Q, F, d_u, d_i, n, d_out, d_bias, U, I);
     DRB_CUDA(cudaGetLastError());
     return DRB_OK;
 }

@@ -211,13 +211,6 @@ __global__ void explode_pointwise_kernel(const int32_t *__restrict__ coo_u, cons
     }
 }
 
-static int grid_for(long long n, int block)
-{
-    long long b = (n + block - 1) / block, cap = (long long)sm_count() * 16;
-    if (b > cap) b = cap;
-    return (int)(b < 1 ? 1 : b);
-}
-
 }  // namespace drb
 
 using namespace drb;

@@ -69,35 +69,37 @@ inline size_t carve(void *base, int U, int I, int F, int opt, Workspace *w, int 
     return off;
 }
 
+// The kernels take StepParams by value: its member order and types are the kernel parameter layout.  Every member has a
+// default: together they describe a fused (phases = 3) BPR step with every model-specific switch off.
 struct StepParams {
-    float *P, *Q;
-    Workspace ws;
-    const int32_t *bu, *bi, *bj;
-    long long n, batch, first_step, n_steps;
-    int U, I, F, tile;
-    float lr, reg1, reg2;
-    int opt;
-    float beta1, beta2, eps;
-    long long adam_step0;
-    double *step_loss;
-    int apply;
-    int phases;      // bit 0: phase 1 (accumulate), bit 1: phase 2 (apply); 3 = fused persistent steps
-    int dense_hint;  // -1 auto, 0 claim, 1 dense sweep (multi-GPU: always dense, counters are global)
+    float *P = nullptr, *Q = nullptr;
+    Workspace ws = {};
+    const int32_t *bu = nullptr, *bi = nullptr, *bj = nullptr;
+    long long n = 0, batch = 0, first_step = 0, n_steps = 0;
+    int U = 0, I = 0, F = 0, tile = 0;   // tile: set by the launcher before every launch
+    float lr = 0.f, reg1 = 0.f, reg2 = 0.f;
+    int opt = DRB_OPT_SGD;
+    float beta1 = 0.f, beta2 = 0.f, eps = 0.f;
+    long long adam_step0 = 0;
+    double *step_loss = nullptr;
+    int apply = 1;
+    int phases = 3;       // bit 0: phase 1 (accumulate), bit 1: phase 2 (apply); 3 = fused persistent steps
+    int dense_hint = -1;  // -1 auto, 0 claim, 1 dense sweep (multi-GPU: always dense, counters are global)
     // LightGCN: scores come from the propagated tables P,Q while the regulariser norms use the ego tables
-    const float *Pn, *Qn;  // ego (norm) tables; nullptr = same as P,Q
-    float gscale;          // factor applied to the accumulated gradient in phase 2 (1/(L+1) for LightGCN)
-    int dense_grad;        // 1: every row has a gradient (propagated), not only the rows a triple touched
+    const float *Pn = nullptr, *Qn = nullptr;  // ego (norm) tables; nullptr = same as P,Q
+    float gscale = 1.f;    // factor applied to the accumulated gradient in phase 2 (1/(L+1) for LightGCN)
+    int dense_grad = 0;    // 1: every row has a gradient (propagated), not only the rows a triple touched
     // NeuMF: the item-side regulariser counts the negative occurrences 2x (GMF table) or 0x (MLP table)
-    float neg_mult;        // multiplier of the negative-occurrence count in the regulariser gradient
-    int keep_counts;       // 1: leave the row counters untouched (another table pair still needs them)
+    float neg_mult = 1.f;  // multiplier of the negative-occurrence count in the regulariser gradient
+    int keep_counts = 0;   // 1: leave the row counters untouched (another table pair still needs them)
     // Fused negative sampling (throughput mode, NOT the reference's per-user-once table): when neg_row_ptr != nullptr the
     // negative of triple t of step s is drawn inside phase 1: k = Philox(seed; t, step) scaled to [0, I - deg(u)), then
     // the k-th item outside the user's sorted CSR row (same complement distribution as sampler.py:86, fresh every step).
-    const int64_t *neg_row_ptr;
-    const int32_t *neg_col;
-    int32_t *neg_out;      // optional: the drawn negatives are written here (aligned with bu/bi) for inspection
-    unsigned long long neg_seed;
-    int loss;              // DRB_LOSS_BPR / _HL / _TL (pair-wise criterion, AbstractRecommender.py:79-93)
+    const int64_t *neg_row_ptr = nullptr;
+    const int32_t *neg_col = nullptr;
+    int32_t *neg_out = nullptr;  // optional: the drawn negatives are written here (aligned with bu/bi) for inspection
+    unsigned long long neg_seed = 0;
+    int loss = DRB_LOSS_BPR;     // DRB_LOSS_BPR / _HL / _TL (pair-wise criterion, AbstractRecommender.py:79-93)
     // FM (FMRecommender.py:61-68): pred += (u_bias[u] + i_bias[item]) + bias_; bias = packed [U + I + 1]; nullptr = MF
     float *bias = nullptr;
     // deterministic accumulation: run-to-run bitwise reproducible steps (fixed-point int64 atomics, see Workspace); single GPU,
@@ -108,6 +110,20 @@ struct StepParams {
     const long long *step_offsets = nullptr;
 };
 
+// One step on a batch of B triples (bu, bi, bj) of a U x I problem with F factors, with the hyper-parameters of h; the
+// optimiser's step counter stands at adam_step0.  The caller adds the tables, the workspace and its model's switches.
+inline StepParams one_step(const drb_hyper *h, int U, int I, int F, const int32_t *bu, const int32_t *bi, const int32_t *bj,
+                           long long B, long long adam_step0)
+{
+    StepParams p;
+    p.bu = bu; p.bi = bi; p.bj = bj;
+    p.n = B; p.batch = B; p.first_step = 0; p.n_steps = 1;
+    p.U = U; p.I = I; p.F = F;
+    p.lr = h->lr; p.reg1 = h->reg_1; p.reg2 = h->reg_2; p.opt = h->opt;
+    p.beta1 = h->beta1; p.beta2 = h->beta2; p.eps = h->eps; p.loss = h->loss;
+    p.adam_step0 = adam_step0;
+    return p;
+}
 
 int fill_params(StepParams &p, float *P, float *Q, void *d_ws, int U, int I, int F, const int32_t *bu, const int32_t *bi,
                 const int32_t *bj, long long n, long long batch, long long first, long long nsteps, const drb_hyper *h,

@@ -98,8 +98,6 @@ def sampler_draw_mt19937(state, row_ptr, user_num, item_num, num_ng):
     bad = C.c_int32(-1)
     rc = L.lib().drb_sampler_draw_mt19937(state.ctypes.data, row_ptr.ctypes.data, user_num, item_num, num_ng,
                                           draws.ctypes.data, C.byref(bad))
-    if rc == L.DRB_ERR_EMPTY_SET:
-        raise ValueError("'a' cannot be empty unless no samples are taken")
     L.check(rc)
     return draws
 
@@ -142,8 +140,6 @@ def sample_triples_host(state, row_ptr, col, coo_u, coo_i, user_num, item_num, n
     rc = L.lib().drb_sample_triples_host(state.ctypes.data, row_ptr.ctypes.data, col.ctypes.data, coo_u.ctypes.data,
                                          coo_i.ctypes.data, len(coo_u), user_num, item_num, num_ng, js.ctypes.data,
                                          tr.ctypes.data, C.byref(bad))
-    if rc == L.DRB_ERR_EMPTY_SET:
-        raise ValueError("'a' cannot be empty unless no samples are taken")
     L.check(rc)
     return js, tr
 
@@ -156,8 +152,6 @@ def bounded_draws_mt19937(state, n, offsets):
     bad = C.c_int64(-1)
     rc = L.lib().drb_bounded_draws_mt19937(state.ctypes.data, n.ctypes.data, offsets.ctypes.data, len(n),
                                            draws.ctypes.data, C.byref(bad))
-    if rc == L.DRB_ERR_EMPTY_SET:
-        raise ValueError("'a' cannot be empty unless no samples are taken")
     L.check(rc)
     return draws
 
@@ -179,8 +173,6 @@ def sampler_draw_mt19937_mixed(state, row_ptr, user_num, item_num, uniform_num, 
     bad = C.c_int32(-1)
     rc = L.lib().drb_sampler_draw_mt19937_mixed(state.ctypes.data, row_ptr.ctypes.data, user_num, item_num, uniform_num,
                                                 other_num, draws.ctypes.data, u01.ctypes.data, C.byref(bad))
-    if rc == L.DRB_ERR_EMPTY_SET:
-        raise ValueError("'a' cannot be empty unless no samples are taken")
     L.check(rc)
     return draws, u01
 
@@ -334,8 +326,6 @@ def mf_bpr_train_steps(P, Q, ws, bu, bi, bj, batch, first_step, n_steps, hp, ada
     fn = L.lib().drb_mf_bpr_train_steps_det if getattr(ws, "det", False) else L.lib().drb_mf_bpr_train_steps
     rc = fn(_ptr(P), _ptr(Q), _ptr(ws.buf), ws.U, ws.I, ws.F, _ptr(bu), _ptr(bi), _ptr(bj), n, batch, first_step, n_steps,
             C.byref(hp), adam_step0, _ptr(losses), 1 if check else 0, C.byref(nan_step), _stream())
-    if rc == L.DRB_ERR_NAN_LOSS:
-        raise ValueError("Loss=Nan or Infinity: current settings does not fit the recommender")
     L.check(rc)
     return losses[:n_steps]
 
@@ -353,8 +343,6 @@ def mf_bpr_train_steps_fused_neg(P, Q, ws, bu, bi, d_row_ptr, d_col, seed, batch
                                                   None if neg_out is None else _ptr(neg_out), bu.numel(), batch, first_step,
                                                   n_steps, C.byref(hp), adam_step0, _ptr(losses), 1 if check else 0,
                                                   C.byref(nan_step), _stream())
-    if rc == L.DRB_ERR_NAN_LOSS:
-        raise ValueError("Loss=Nan or Infinity: current settings does not fit the recommender")
     L.check(rc)
     return losses[:n_steps]
 
@@ -380,8 +368,6 @@ def mf_bpr_train_step_host(P, Q, ws, h_bu, h_bi, h_bj, hp, stage, adam_step0=0):
     loss = C.c_double(0.0)
     rc = L.lib().drb_mf_bpr_train_step_host(_ptr(P), _ptr(Q), _ptr(ws.buf), ws.U, ws.I, ws.F, hp_(h_bu), hp_(h_bi),
                                             hp_(h_bj), n, C.byref(hp), adam_step0, _ptr(stage), C.byref(loss), _stream())
-    if rc == L.DRB_ERR_NAN_LOSS:
-        raise ValueError("Loss=Nan or Infinity: current settings does not fit the recommender")
     L.check(rc)
     return loss.value
 
@@ -400,8 +386,6 @@ def mf_bpr_train_steps_host(P, Q, ws, h_bu, h_bi, h_bj, batch, n_steps, hp, adam
     rc = L.lib().drb_mf_bpr_train_steps_host(_ptr(P), _ptr(Q), _ptr(ws.buf), ws.U, ws.I, ws.F, h_bu.data_ptr(),
                                              h_bi.data_ptr(), h_bj.data_ptr(), n, batch, n_steps, C.byref(hp), adam_step0,
                                              _ptr(stage), _ptr(d_loss), h_loss.data_ptr(), C.byref(nan_step), _stream())
-    if rc == L.DRB_ERR_NAN_LOSS:
-        raise ValueError("Loss=Nan or Infinity: current settings does not fit the recommender")
     L.check(rc)
     return h_loss[:n_steps]
 
@@ -429,8 +413,6 @@ def fm_train_steps(P, Q, bias, ws, bu, bi, bj, batch, first_step, n_steps, hp, a
     rc = L.lib().drb_fm_train_steps(_ptr(P), _ptr(Q), _ptr(bias), _ptr(ws.buf), ws.U, ws.I, ws.F, _ptr(bu), _ptr(bi), _ptr(bj),
                                     bu.numel(), batch, first_step, n_steps, C.byref(hp), adam_step0, 1 if apply else 0,
                                     _ptr(losses), 1 if check else 0, C.byref(nan_step), _stream())
-    if rc == L.DRB_ERR_NAN_LOSS:
-        raise ValueError("Loss=Nan or Infinity: current settings does not fit the recommender")
     L.check(rc)
     return losses[:n_steps]
 
@@ -567,8 +549,6 @@ def lgcn_bpr_train_steps(E0, ws, graph, num_layers, bu, bi, bj, batch, first_ste
                                           _ptr(bi), _ptr(bj), bu.numel(), batch, first_step, n_steps, C.byref(hp),
                                           adam_step0, 1 if apply else 0, _ptr(losses), 1 if check else 0,
                                           C.byref(nan_step), _stream())
-    if rc == L.DRB_ERR_NAN_LOSS:
-        raise ValueError("Loss=Nan or Infinity: current settings does not fit the recommender")
     L.check(rc)
     return losses[:n_steps]
 
@@ -630,8 +610,6 @@ def ngcf_bpr_train_steps(E0, W, ws, graph, bu, bi, bj, batch, first_step, n_step
                                                   None if keep is None else _ptr(keep),
                                                   C.c_float(dropout if keep is not None else 0.0), _ptr(losses),
                                                   1 if check else 0, C.byref(nan_step), _stream())
-    if rc == L.DRB_ERR_NAN_LOSS:
-        raise ValueError("Loss=Nan or Infinity: current settings does not fit the recommender")
     L.check(rc)
     return losses[:n_steps]
 
@@ -676,8 +654,6 @@ def nfm_bpr_train_steps(P, Q, bias, N, Rs, ws, act, bu, bi, bj, batch, first_ste
         ws.Ln, ws.bn, act, ws.max_rows, _ptr(bu), _ptr(bi), _ptr(bj), bu.numel(), batch, first_step, n_steps, C.byref(hp), adam_step0,
         1 if apply else 0, tower_dtype, None if keep is None else _ptr(keep), C.c_float(dropout if keep is not None else 0.0),
         _ptr(losses), 1 if check else 0, C.byref(nan_step), _stream())
-    if rc == L.DRB_ERR_NAN_LOSS:
-        raise ValueError("Loss=Nan or Infinity: current settings does not fit the recommender")
     L.check(rc)
     return losses[:n_steps]
 
@@ -735,8 +711,6 @@ def neumf_bpr_train_steps(tabs, W, ws, bu, bi, bj, batch, first_step, n_steps, h
                                            tower_dtype, C.c_float(dropout), C.c_uint64(dropout_seed),
                                            None if drop_masks is None else _ptr(drop_masks), mode, _ptr(losses),
                                            1 if check else 0, C.byref(nan_step), _stream())
-    if rc == L.DRB_ERR_NAN_LOSS:
-        raise ValueError("Loss=Nan or Infinity: current settings does not fit the recommender")
     L.check(rc)
     return losses[:n_steps]
 

@@ -383,7 +383,7 @@ class ShardedTrainer:
         hdr = self.ws.buf[:256].cpu().numpy()
         status = int(np.frombuffer(hdr[144:148].tobytes(), np.int32)[0])   # WsHeader: barrier 8 + acc 128 + nan_step 8
         if status == L.DRB_ERR_NAN_LOSS:
-            raise ValueError("Loss=Nan or Infinity: current settings does not fit the recommender")
+            raise ValueError(L.NAN_LOSS_MESSAGE)
         if status == L.DRB_ERR_PEER:
             raise RuntimeError("multi-GPU peer exchange timed out: a rank did not reach the rendezvous (see DESIGN.md, "
                                "multi-GPU section); the NCCL step (sharded_comm='nccl') is the fallback")
