@@ -37,6 +37,7 @@ SIGNATURES = {
     "drb_index_range_check": (C.c_int, [vp, C.c_int32, C.c_int64, C.c_int32, c_i64p, c_i64p, vp]),
     "drb_mf_step_variant": (C.c_int, [C.c_int32, C.c_int64, C.POINTER(C.c_int32), C.POINTER(C.c_int32)]),
     "drb_mf_step_selfcheck_ms": (C.c_int, [C.c_int32, C.c_int64, C.POINTER(C.c_float), C.POINTER(C.c_float), C.POINTER(C.c_int32)]),
+    "drb_mf_last_step_mode": (C.c_int, []),
     "drb_mf_step_geometry": (C.c_int, [C.c_int32, C.c_int32, C.POINTER(C.c_int32), C.POINTER(C.c_int32), C.c_int64,
                                        C.POINTER(C.c_int32)]),
     "drb_mt19937_seed": (C.c_int, [vp, C.c_uint32]),

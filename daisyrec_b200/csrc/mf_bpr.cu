@@ -32,6 +32,7 @@
 #include <math.h>
 #include <stdlib.h>
 
+#include <atomic>
 #include <map>
 #include <mutex>
 #include <vector>
@@ -127,6 +128,75 @@ static StepKernel pick_lean_wn(int W, int NCH)
 #undef DRB_LEAN
     return nullptr;
 }
+// the user-bucketed mode of the lean kernel: instantiated for the preferred geometries of F = 32 and 64 (8 lanes x 1 or 2 chunks);
+// at 8 x 4 (F = 128) it spills under the 128-register bound of two resident CTAs per SM
+static StepKernel pick_lean_ub(int W, int NCH)
+{
+    if (W != 8) return nullptr;
+    if (NCH == 1) return mf_bpr_steps_lean_kernel<4, 8, 1, true>;
+    if (NCH == 2) return mf_bpr_steps_lean_kernel<4, 8, 2, true>;
+    return nullptr;
+}
+static int ubucket_switch()
+{
+    static const int v = [] {
+        const char *e = getenv("DRB_UBUCKET");   // developer switch: 0 forbids the user-bucketed mode, 1 forces it (once checked)
+        return e ? (atoi(e) != 0 ? 1 : 0) : -1;
+    }();
+    return v;
+}
+
+// Users per bucket of the user-bucketed mode: about 8 buckets per resident CTA, so that the dynamic claiming of buckets balances
+// the phase (bucket sizes follow the user degrees); at least kUbMinUsers, at most what a 64 KB shared accumulator holds.  0 when
+// the mode cannot run the problem (more than kUbMaxBuckets buckets: the per-CTA histogram would not fit shared memory).
+constexpr int kUbMinUsers = 16, kUbMaxBuckets = 8192;
+constexpr long long kUbTimedBatch = 1 << 19;   // triples per step of the on-device timing problem (lean_autotune)
+static int ub_users_for(int U, int F, long long batch)
+{
+    const int target = 8 * DRB_MINB * sm_count();
+    int ub = (U + target - 1) / target;
+    if (ub < kUbMinUsers) ub = kUbMinUsers;
+    const int cap = 65536 / ((F + 1) * 4 + 4);
+    if (ub > cap) ub = cap;
+    if (ub < 1) return 0;
+    const long long nbk = ((long long)U + ub - 1) / ub;
+    return (nbk <= kUbMaxBuckets && batch + 4 * nbk < (1LL << 31)) ? ub : 0;
+}
+
+// The bucketed mode's scratch (counters, bucket ranges, partitioned planes): library-owned, grow-only, one per device and stream;
+// it depends on the batch, so it cannot live in the workspace.  Its counters are cleared before every launch.  Each buffer lives
+// as long as the process: about 12 B x the largest batch of bucketed steps launched on that stream (12.6 MB at B = 1 M), so a
+// caller that trains on many streams holds one such buffer per stream.
+static int ub_scratch(StepParams &p, cudaStream_t st)
+{
+    static std::mutex mu;
+    static std::map<std::pair<int, cudaStream_t>, std::pair<void *, size_t>> bufs;
+    const size_t nbk = (size_t)p.ub_buckets;
+    const size_t cnt_b = align256(sizeof(unsigned) * (2 * nbk + 1)), rng_b = align256(sizeof(int) * 2 * nbk);
+    const size_t plane = align256(sizeof(int32_t) * ((size_t)p.batch + 4 * nbk));
+    const size_t need = cnt_b + rng_b + 3 * plane;
+    int dev = 0;
+    DRB_CUDA(cudaGetDevice(&dev));
+    std::lock_guard<std::mutex> lock(mu);
+    auto &e = bufs[std::make_pair(dev, st)];
+    if (e.second < need) {
+        if (e.first != nullptr) {
+            DRB_CUDA(cudaStreamSynchronize(st));   // an earlier launch on this stream may still read it
+            DRB_CUDA(cudaFree(e.first));
+            e = std::make_pair(nullptr, (size_t)0);
+        }
+        DRB_CUDA(cudaMalloc(&e.first, need));
+        e.second = need;
+    }
+    char *b = (char *)e.first;
+    p.ub_count = (unsigned *)b;
+    p.ub_range = (int *)(b + cnt_b);
+    p.ub_u = (int32_t *)(b + cnt_b + rng_b);
+    p.ub_i = (int32_t *)(b + cnt_b + rng_b + plane);
+    p.ub_j = (int32_t *)(b + cnt_b + rng_b + 2 * plane);
+    DRB_CUDA(cudaMemsetAsync(p.ub_count, 0, sizeof(unsigned) * (2 * nbk + 1), st));
+    return DRB_OK;
+}
 
 // GEN = false: BPR only (the hot instantiation, no loss-kind branches); GEN = true: HL / TL selected at run time
 static StepKernel pick_kernel(int F, bool gen)
@@ -144,16 +214,35 @@ static StepKernel pick_kernel(int F, bool gen)
 }
 
 // grid / tile choice and the cooperative launch of one chosen instantiation
-static int launch_kernel(StepKernel k, StepParams &p, cudaStream_t st, bool keep_status, int tile_cap = kTileDefault)
+// (ub: k is a user-bucketed instantiation; the launch sizes its buckets, scratch and dynamic shared memory)
+static int launch_kernel(StepKernel k, StepParams &p, cudaStream_t st, bool keep_status, int tile_cap = kTileDefault,
+                         bool ub = false)
 {
-    // occupancy of the chosen instantiation, cached (the query costs microseconds and this runs once per step in the
-    // split multi-GPU / LightGCN / NeuMF paths)
+    size_t smem = 0;
+    if (ub) {
+        p.ub_users = ub_users_for(p.U, p.F, p.batch);
+        DRB_REQUIRE(p.ub_users > 0, "user-bucketed step: %d users in more than %d buckets", p.U, kUbMaxBuckets);
+        p.ub_buckets = (p.U + p.ub_users - 1) / p.ub_users;
+        const size_t acc = sizeof(float) * (size_t)p.ub_users * (p.F + 1) + sizeof(unsigned) * p.ub_users;
+        const size_t hist = 2 * sizeof(unsigned) * (size_t)p.ub_buckets;
+        smem = ((acc > hist ? acc : hist) + 15) / 16 * 16;
+        const int rc = ub_scratch(p, st);
+        if (rc != DRB_OK) return rc;
+    }
+    // occupancy of the chosen instantiation, cached per device (the query costs microseconds and this runs once per step in the
+    // split multi-GPU / LightGCN / NeuMF paths); the dynamic shared-memory limit is a per-device function attribute
     static thread_local StepKernel cached_k = nullptr;
-    static thread_local int cached_per_sm = 0;
-    if (cached_k != k) {
+    static thread_local size_t cached_smem = 0;
+    static thread_local int cached_dev = -1, cached_per_sm = 0;
+    int dev = 0;
+    DRB_CUDA(cudaGetDevice(&dev));
+    if (cached_k != k || cached_smem != smem || cached_dev != dev) {
         int q = 0;
-        DRB_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&q, k, kThreads, 0));
+        if (smem > 0) DRB_CUDA(cudaFuncSetAttribute((const void *)k, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+        DRB_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&q, k, kThreads, smem));
         cached_k = k;
+        cached_smem = smem;
+        cached_dev = dev;
         cached_per_sm = q;
     }
     const int per_sm = cached_per_sm;
@@ -171,7 +260,7 @@ static int launch_kernel(StepKernel k, StepParams &p, cudaStream_t st, bool keep
     if (p.phases & 1)
         DRB_CUDA(cudaMemsetAsync(p.ws.hdr, 0, (p.phases == 3 && !keep_status) ? sizeof(WsHeader) : kHdrResetBytes, st));
     void *args[] = {&p};
-    DRB_CUDA(cudaLaunchCooperativeKernel((void *)k, dim3(grid), dim3(kThreads), args, 0, st));
+    DRB_CUDA(cudaLaunchCooperativeKernel((void *)k, dim3(grid), dim3(kThreads), args, smem, st));
     return DRB_OK;
 }
 
@@ -202,7 +291,7 @@ static void make_check_problem(CheckProblem &c, int U, int I, int F, int B, int 
 // one launch of K steps of instantiation k on a fresh copy of the problem; optional outputs: tables, losses, milliseconds of a
 // second (warm) launch
 static bool run_check_variant(const CheckProblem &c, StepKernel k, int opt, float lr, std::vector<float> *outP,
-                              std::vector<float> *outQ, double *loss, float *ms, int tile_cap = kTileDefault)
+                              std::vector<float> *outQ, double *loss, float *ms, int tile_cap = kTileDefault, bool ub = false)
 {
     const long long n = (long long)c.B * c.K;
     const size_t wsb = carve(nullptr, c.U, c.I, c.F, opt, nullptr);
@@ -226,14 +315,14 @@ static bool run_check_variant(const CheckProblem &c, StepKernel k, int opt, floa
         drb_hyper h = {lr, 0.001f, 0.001f, opt, 0.9f, 0.999f, 1e-8f, DRB_LOSS_BPR};
         StepParams p;
         good = fill_params(p, dP, dQ, dws, c.U, c.I, c.F, du, di, dj, n, c.B, 0, c.K, &h, 0, dl, 1) == DRB_OK &&
-               launch_kernel(k, p, (cudaStream_t)0, false, tile_cap) == DRB_OK &&
+               launch_kernel(k, p, (cudaStream_t)0, false, tile_cap, ub) == DRB_OK &&
                cudaStreamSynchronize((cudaStream_t)0) == cudaSuccess;
         if (good && ms != nullptr) {
             *ms = 0.f;
             for (int rep = 0; rep < 2 && good; ++rep) {            // best of two warm launches
                 float t = 0.f;
                 cudaEventRecord(e0, (cudaStream_t)0);
-                good = launch_kernel(k, p, (cudaStream_t)0, false, tile_cap) == DRB_OK;
+                good = launch_kernel(k, p, (cudaStream_t)0, false, tile_cap, ub) == DRB_OK;
                 cudaEventRecord(e1, (cudaStream_t)0);
                 good = good && cudaEventSynchronize(e1) == cudaSuccess && cudaEventElapsedTime(&t, e0, e1) == cudaSuccess;
                 if (good && (rep == 0 || t < *ms)) *ms = t;
@@ -257,8 +346,22 @@ static bool run_check_variant(const CheckProblem &c, StepKernel k, int opt, floa
 struct LeanChoice {
     int W = 0, NCH = 0;               // lanes per row, chunks per lane of the lean instantiation; W == 0: the general one
     int tile_cap = kTileDefault;
-    float ms_general = 0.f, ms_lean = 0.f;   // timed launch of the autotune (best lean candidate)
+    int ub_W = 0, ub_NCH = 0;         // geometry of the user-bucketed mode when it was selected (it then runs the fused steps)
+    float ms_general = 0.f, ms_lean = 0.f;   // timed launch of the autotune (the lean kernel that runs: best lean candidate or
+                                             // the bucketed mode)
 };
+
+// the user-bucketed mode's edge cases: several buckets, U not a multiple of the bucket width, an empty bucket (2), and one user
+// with more triples in a step than an index tile holds (run at lr 0.01: at 0.05 its large item sums leave the fp32 noise of the
+// general kernel alone near the 1e-5 table tolerance)
+static void make_bucket_problem(CheckProblem &c, int F)
+{
+    make_check_problem(c, 5 * kUbMinUsers + 7, 64, F, 3000, 2, false);
+    for (size_t t = 0; t < c.hu.size(); ++t) {
+        if (t % 5 < 2) c.hu[t] = 3;                                           // 1 200 triples of user 3 per step
+        else if (c.hu[t] / kUbMinUsers == 2) c.hu[t] += kUbMinUsers;
+    }
+}
 
 // same losses (1e-5 rel) and tables (1e-5 abs) as the reference outputs of the general instantiation
 static bool same_results(const CheckProblem &c, int opt, const std::vector<float> &P0, const std::vector<float> &Q0,
@@ -317,7 +420,7 @@ static LeanChoice lean_autotune(int F, bool hbm)
     // left to the streamed index planes); for the HBM regime 2 x 134 MB of user rows
     const long long l2_rows = l2_bytes() / (2LL * 8 * F) * 4 / 5;
     const int rows = hbm ? 33554432 / F : (int)(l2_rows > 4096 ? l2_rows : 4096);
-    make_check_problem(big, rows, hbm ? 16384 : rows / 4, F, 1 << 19, 3, false);
+    make_check_problem(big, rows, hbm ? 16384 : rows / 4, F, (int)kUbTimedBatch, 3, false);
     std::vector<float> refP[2], refQ[2];
     double refl[2][2];
     bool ok = true;
@@ -352,15 +455,47 @@ static LeanChoice lean_autotune(int F, bool hbm)
             fprintf(stderr, "[daisyrec_b200] lean step kernel (factors=%d): %.3f ms against %.3f ms of the general instantiation on "
                             "the timing problem: keeping the general one\n", F, best_ms, best.ms_general);
         best.W = best.NCH = 0;
-        return best;
+    } else {
+        float ms_big_tile = 0.f;                                  // a larger index tile for the chosen candidate?
+        if (run_check_variant(big, pick_lean_wn(best.W, best.NCH), DRB_OPT_SGD, 0.01f, nullptr, nullptr, nullptr, &ms_big_tile,
+                              kTileMax) && ms_big_tile > 0.f && ms_big_tile < 0.98f * best_ms) {
+            best.tile_cap = kTileMax;
+            best.ms_lean = ms_big_tile;
+        }
+        cudaGetLastError();
     }
-    float ms_big_tile = 0.f;                                      // a larger index tile for the chosen candidate?
-    if (run_check_variant(big, pick_lean_wn(best.W, best.NCH), DRB_OPT_SGD, 0.01f, nullptr, nullptr, nullptr, &ms_big_tile,
-                          kTileMax) && ms_big_tile > 0.f && ms_big_tile < 0.98f * best_ms) {
-        best.tile_cap = kTileMax;
-        best.ms_lean = ms_big_tile;
+    // The user-bucketed mode (preferred geometry): the same two checks on the small problem and on its edge-case problem, then
+    // timed on the regime's problem; it runs if it beats what would run otherwise by 2 % (or DRB_UBUCKET=1).
+    StepKernel ub = pick_lean_ub(cw[0], cn[0]);
+    if (!ok || ub == nullptr || ubucket_switch() == 0) return best;
+    CheckProblem edge;
+    make_bucket_problem(edge, F);
+    bool same = true;
+    for (int opt = DRB_OPT_SGD; opt <= DRB_OPT_ADAM && same; ++opt) {
+        std::vector<float> P0, Q0, P1, Q1;
+        double l0[2], l1[2];
+        same = run_check_variant(small, ub, opt, 0.05f, &P1, &Q1, l1, nullptr, kTileDefault, true) &&
+               same_results(small, opt, refP[opt], refQ[opt], refl[opt], P1, Q1, l1) &&
+               run_check_variant(edge, gen, opt, 0.01f, &P0, &Q0, l0, nullptr) &&
+               run_check_variant(edge, ub, opt, 0.01f, &P1, &Q1, l1, nullptr, kTileDefault, true) &&
+               same_results(edge, opt, P0, Q0, l0, P1, Q1, l1);
     }
     cudaGetLastError();
+    if (!same) {
+        fprintf(stderr, "[daisyrec_b200] user-bucketed step kernel (factors=%d) did not reproduce the general instantiation: not "
+                        "used\n", F);
+        return best;
+    }
+    float ms = 0.f;
+    const bool timed = run_check_variant(big, ub, DRB_OPT_SGD, 0.01f, nullptr, nullptr, nullptr, &ms, best.tile_cap, true) &&
+                       ms > 0.f;
+    cudaGetLastError();
+    const float current = best.W > 0 ? best.ms_lean : best.ms_general;
+    if (timed && (ubucket_switch() == 1 || ms < 0.98f * current)) {
+        best.ub_W = cw[0];
+        best.ub_NCH = cn[0];
+        best.ms_lean = ms;
+    }
     return best;
 }
 
@@ -393,16 +528,29 @@ void lean_geom(int F, long long table_rows, int &W, int &NCH)
 }
 int lean_tile_cap(int F, long long table_rows) { return lean_choice(F, table_rows).tile_cap; }
 
+// which instantiation the last launch_steps call of any thread ran: 0 general, 1 lean, 2 lean user-bucketed
+static std::atomic<int> g_last_step_mode{0};
+
 int launch_steps(StepParams &p, cudaStream_t st, bool keep_status)
 {
     // lean: the MF hot path; GEN: any loss but BPR, Adagrad / RMSprop sweeps, FM biases, deterministic accumulation
     StepKernel k = nullptr;
-    int tile_cap = kTileDefault;
+    int tile_cap = kTileDefault, mode = 0;
+    bool ub = false;
     if (step_params_lean(p)) {
         const LeanChoice &c = lean_choice(p.F, (long long)p.U + p.I);
-        if (c.W > 0) {
+        // user-bucketed mode: single-GPU fused steps over uniform batches that update the tables, at least as large as the
+        // batch it was timed at (its per-step partition is not amortised by small batches); DRB_UBUCKET=1 takes it at any size
+        if (c.ub_W > 0 && p.phases == 3 && p.step_offsets == nullptr && p.apply == 1 && ub_users_for(p.U, p.F, p.batch) > 0 &&
+            (p.batch >= kUbTimedBatch || ubucket_switch() == 1)) {
+            k = pick_lean_ub(c.ub_W, c.ub_NCH);
+            tile_cap = c.tile_cap;
+            ub = true;
+            mode = 2;
+        } else if (c.W > 0) {
             k = pick_lean_wn(c.W, c.NCH);
             tile_cap = c.tile_cap;
+            mode = 1;
         }
     }
     if (k == nullptr) {
@@ -412,7 +560,8 @@ int launch_steps(StepParams &p, cudaStream_t st, bool keep_status)
     DRB_REQUIRE(!p.det || (p.phases == 3 && p.ws.gP64 != nullptr), "deterministic accumulation: single-GPU fused steps with a "
                 "workspace from drb_mf_workspace_bytes_det");
     DRB_REQUIRE(k != nullptr, "unsupported factors=%d (row too long for 32 lanes x 8 chunks)", p.F);
-    return launch_kernel(k, p, st, keep_status, tile_cap);
+    g_last_step_mode = mode;
+    return launch_kernel(k, p, st, keep_status, tile_cap, ub);
 }
 
 int check_nan(void *d_ws, cudaStream_t st, int64_t *nan_step)
@@ -438,12 +587,13 @@ extern "C" size_t drb_mf_workspace_bytes(int32_t U, int32_t I, int32_t F, int32_
     return carve(nullptr, U, I, F, opt, nullptr);
 }
 
-// 1: BPR + SGD/Adam steps at this factor count run the lean instantiation (after its self-check), 0: the general one.
-// lanes / chunks (optional) receive the lane geometry of that instantiation.
+// 1: BPR + SGD/Adam steps at this factor count run the lean instantiation (after its self-check), 2: its user-bucketed mode
+// (single-GPU fused steps), 0: the general one.  lanes / chunks (optional) receive the lane geometry of that instantiation.
 extern "C" int drb_mf_step_variant(int32_t F, int64_t table_rows, int32_t *lanes, int32_t *chunks)
 {
-    int W = 0, NCH = 0;
-    drb::lean_geom(F, table_rows, W, NCH);
+    const drb::LeanChoice &c = drb::lean_choice(F, table_rows);
+    const bool bucketed = c.ub_W > 0;
+    int W = bucketed ? c.ub_W : c.W, NCH = bucketed ? c.ub_NCH : c.NCH;
     const bool lean = W > 0;
     if (!lean && F > 0) {
         drb::RowGeom g = drb::row_geom(F);
@@ -452,8 +602,12 @@ extern "C" int drb_mf_step_variant(int32_t F, int64_t table_rows, int32_t *lanes
     }
     if (lanes) *lanes = W;
     if (chunks) *chunks = NCH;
-    return lean ? 1 : 0;
+    return bucketed ? 2 : lean ? 1 : 0;
 }
+
+// which instantiation the last BPR step launch ran: 0 general, 1 lean, 2 lean user-bucketed (a launch-time choice: the bucketed
+// mode also depends on the launch's batch and phases)
+extern "C" int drb_mf_last_step_mode(void) { return drb::g_last_step_mode; }
 
 // the timing half of the on-device selection for `factors`: milliseconds of the timed launch (3 steps of 524 288 triples) of the
 // general instantiation and of the best lean candidate, and the index-tile cap in use (runs the selection if it has not run)

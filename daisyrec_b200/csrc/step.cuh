@@ -108,6 +108,12 @@ struct StepParams {
     // multi-GPU persistent mode: step s trains local triples [step_offsets[s], step_offsets[s+1]) (device array; the union
     // of the ranks' ranges is the global batch s).  nullptr = uniform batches of `batch` triples.
     const long long *step_offsets = nullptr;
+    // user-bucketed phase 1 (lean single-GPU fused steps only): bucket b holds users [b * ub_users, (b + 1) * ub_users).  Scratch
+    // owned by the launcher (mf_bpr.cu), not part of the workspace: its size depends on the batch.
+    int ub_users = 0, ub_buckets = 0;
+    unsigned *ub_count = nullptr;  // [2 * ub_buckets + 1]: triples per bucket, reservation cursors, work counter; zero between steps
+    int *ub_range = nullptr;       // [2 * ub_buckets]: first and end position of bucket b in the partitioned planes
+    int32_t *ub_u = nullptr, *ub_i = nullptr, *ub_j = nullptr;  // partitioned planes; every bucket starts at a multiple of 4
 };
 
 // One step on a batch of B triples (bu, bi, bj) of a U x I problem with F factors, with the hyper-parameters of h; the

@@ -264,10 +264,17 @@ struct NoExchange {
 // LEAN: the MF hot instantiation (launch_steps picks it when the parameters allow): BPR, no ego / norm tables (LightGCN),
 // no in-kernel negative draw, and 32-bit element offsets into the tables (rows * F < 2^32) -- the same arithmetic on the same
 // operands in the same order as the general body, with ~1/3 fewer instructions per triple.
-template <int VEC, int W, int NCH, bool GEN, class XCH, bool LEAN = false>
+//
+// UBK (user-bucketed, lean single-GPU fused steps only): every step first partitions its triples by user bucket into scratch planes
+// (histogram, grid barrier, scan + reservation, scatter, grid barrier); phase 1 then has CTAs claim whole buckets, sum the user
+// gradient rows and counts of the bucket in shared memory and write each touched gP row and cntU entry once with plain stores,
+// instead of one RED per occurrence into the (L2-missing) user accumulators.  Item side, loss and norms are unchanged; only the
+// fp32 summation order of the user gradient differs (the REDs leave it unspecified as well).
+template <int VEC, int W, int NCH, bool GEN, class XCH, bool LEAN = false, bool UBK = false>
 __device__ __forceinline__ void bpr_steps_body(StepParams &p, XCH &xch)
 {
     static_assert(!(GEN && LEAN), "the lean body is BPR only");
+    static_assert(!UBK || (LEAN && VEC == 4 && !XCH::kActive), "the user-bucketed mode is a single-GPU lean mode");
     using RowOff = typename RowOffset<LEAN>::type;
     constexpr int GPW = 32 / W;                  // lane groups per warp
     constexpr int GROUPS = (kThreads / 32) * GPW;  // lane groups per CTA
@@ -276,6 +283,9 @@ __device__ __forceinline__ void bpr_steps_body(StepParams &p, XCH &xch)
     __shared__ __align__(128) int32_t s_idx[2][3][kTileMax];
     __shared__ uint64_t s_bar[2];
     __shared__ double s_red[8][kThreads / 32];
+    extern __shared__ __align__(16) unsigned char s_dyn[];   // UBK: partition histogram, then the bucket accumulator
+    __shared__ int s_claim[3];                               // UBK: claimed bucket, its first and end position
+    __shared__ unsigned s_wsum[kThreads / 32];               // UBK: per-warp sums of the bucket-count scan
 
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
     const int gl = lane % W, gw = lane / W;
@@ -318,6 +328,28 @@ __device__ __forceinline__ void bpr_steps_body(StepParams &p, XCH &xch)
             if (tid == 0) mbar_arrive(&s_bar[b]);
         }
     };
+    // UBK, thread 0: bulk copy of the partitioned triples [t0, t0 + cnt) into tile buffer b (every bucket starts at a multiple
+    // of 4 triples and has room for the rounding up)
+    auto stage_ub = [&](int t0, int cnt, int b) {
+        const uint32_t bytes = (uint32_t)((cnt + 3) & ~3) * 4u;
+        mbar_expect_tx(&s_bar[b], 3u * bytes);
+        tma_load_1d(&s_idx[b][0][0], p.ub_u + t0, bytes, &s_bar[b]);
+        tma_load_1d(&s_idx[b][1][0], p.ub_i + t0, bytes, &s_bar[b]);
+        tma_load_1d(&s_idx[b][2][0], p.ub_j + t0, bytes, &s_bar[b]);
+    };
+    // UBK, thread 0: claim the next non-empty bucket through the work counter, publish it in s_claim and stage its first tile
+    auto claim = [&](int b) {
+        int k, c0 = 0, c1 = 0;
+        do {
+            k = (int)atomicAdd(p.ub_count + 2 * p.ub_buckets, 1u);
+            if (k < p.ub_buckets) { c0 = __ldcg(p.ub_range + 2 * k); c1 = __ldcg(p.ub_range + 2 * k + 1); }
+        } while (k < p.ub_buckets && c0 == c1);
+        s_claim[0] = k; s_claim[1] = c0; s_claim[2] = c1;
+        if (k < p.ub_buckets) {
+            asm volatile("fence.proxy.async.global;" ::: "memory");   // generic-proxy writes of the planes -> bulk copy
+            stage_ub(c0, min(c1 - c0, kTileMax), b);
+        }
+    };
 
     for (long long s = 0; s < p.n_steps; ++s) {
         const long long step = p.first_step + s;
@@ -334,12 +366,87 @@ __device__ __forceinline__ void bpr_steps_body(StepParams &p, XCH &xch)
         __syncthreads();
         int buf = 0;
         long long t_i = blockIdx.x;
-        if (t_i < ntiles) stage(base + t_i * tile, (int)min((long long)tile, nb - t_i * tile), 0);
-        for (; t_i < ntiles; t_i += gridDim.x) {
-            long long t_n = t_i + gridDim.x;
-            if (t_n < ntiles) stage(base + t_n * tile, (int)min((long long)tile, nb - t_n * tile), buf ^ 1);
+        // UBK: claimed bucket bk, its triples [r0, r1) in the partitioned planes, position tt of the current tile; the gradient
+        // rows and counts of its users u0 .. u0 + rows - 1 sum in s_gp / s_cu (row stride F + 1 against bank conflicts between
+        // the groups of a warp)
+        int bk = 0, r0 = 0, r1 = 0, tt = 0, u0 = 0, rows = 0;
+        float *s_gp = nullptr;
+        unsigned *s_cu = nullptr;
+        if constexpr (UBK) {
+            const int NBK = p.ub_buckets, UBU = p.ub_users, RS = F + 1;
+            unsigned *ucnt = p.ub_count, *ucur = p.ub_count + NBK;
+            // ---- partition: per-CTA histogram of the bucket ids -> global counts
+            unsigned *s_hist = reinterpret_cast<unsigned *>(s_dyn), *s_off = s_hist + NBK;
+            for (int b = tid; b < NBK; b += kThreads) s_hist[b] = 0u;
+            __syncthreads();
+            const long long g0 = (long long)blockIdx.x * kThreads + tid, gstride = (long long)gridDim.x * kThreads;
+            for (long long t = g0; t < nb; t += gstride) atomicAdd(&s_hist[__ldg(p.bu + base + t) / UBU], 1u);
+            __syncthreads();
+            for (int b = tid; b < NBK; b += kThreads)
+                if (s_hist[b] != 0u) red_add_u32(ucnt + b, s_hist[b]);
+            grid_barrier(&hdr->barrier, epoch);
+            // exclusive scan of the counts, each padded to a multiple of 4 (bulk copies of a bucket start 16-byte aligned), in
+            // every CTA; CTA 0 publishes the ranges; each CTA reserves its slice of every bucket it holds triples of
+            const int per = (NBK + kThreads - 1) / kThreads, b0 = min(NBK, tid * per), b1 = min(NBK, b0 + per);
+            unsigned run = 0u;
+            for (int b = b0; b < b1; ++b) run += (__ldcg(ucnt + b) + 3u) & ~3u;
+            unsigned incl = run;
+#pragma unroll
+            for (int off = 1; off < 32; off <<= 1) {
+                const unsigned y = __shfl_up_sync(0xffffffffu, incl, off);
+                if (lane >= off) incl += y;
+            }
+            if (lane == 31) s_wsum[warp] = incl;
+            __syncthreads();
+            unsigned start = incl - run;
+            for (int w = 0; w < warp; ++w) start += s_wsum[w];
+            for (int b = b0; b < b1; ++b) {
+                const unsigned c = __ldcg(ucnt + b), h = s_hist[b];
+                if (blockIdx.x == 0) { p.ub_range[2 * b] = (int)start; p.ub_range[2 * b + 1] = (int)(start + c); }
+                s_off[b] = h != 0u ? start + atomicAdd(ucur + b, h) : 0u;
+                s_hist[b] = 0u;
+                start += (c + 3u) & ~3u;
+            }
+            __syncthreads();
+            // ---- scatter this CTA's triples into the partitioned planes (the same triples as the histogram pass)
+            for (long long t = g0; t < nb; t += gstride) {
+                const int u = __ldg(p.bu + base + t), b = u / UBU;
+                const unsigned pos = s_off[b] + atomicAdd(&s_hist[b], 1u);
+                p.ub_u[pos] = u;
+                p.ub_i[pos] = __ldg(p.bi + base + t);
+                p.ub_j[pos] = __ldg(p.bj + base + t);
+            }
+            asm volatile("fence.proxy.async.global;" ::: "memory");   // the planes are read back by bulk copies (async proxy)
+            grid_barrier(&hdr->barrier, epoch);
+            for (long long k = g0; k < 2LL * NBK; k += gstride) ucnt[k] = 0u;   // counts, cursors: zero for the next step
+            s_gp = reinterpret_cast<float *>(s_dyn);
+            s_cu = reinterpret_cast<unsigned *>(s_gp + UBU * RS);
+            // ---- phase 1 over whole buckets, claimed dynamically (bucket sizes follow the user degrees)
+            if (tid == 0) claim(0);
+            __syncthreads();
+            bk = s_claim[0]; r0 = s_claim[1]; r1 = s_claim[2]; tt = r0;
+        } else {
+            if (t_i < ntiles) stage(base + t_i * tile, (int)min((long long)tile, nb - t_i * tile), 0);
+        }
+        for (; UBK ? bk < p.ub_buckets : t_i < ntiles; t_i += gridDim.x) {
+            if constexpr (UBK) {
+                if (tt == r0) {                                  // first tile of a bucket: zero its accumulator rows
+                    u0 = bk * p.ub_users;
+                    rows = min(p.ub_users, p.U - u0);
+                    for (int k = tid; k < rows * (F + 1); k += kThreads) s_gp[k] = 0.f;
+                    for (int k = tid; k < rows; k += kThreads) s_cu[k] = 0u;
+                    __syncthreads();                             // zeroed; every thread has read s_claim
+                }
+                if (tid == 0) {                                  // prefetch: the bucket's next tile or the next bucket
+                    if (tt + kTileMax < r1) stage_ub(tt + kTileMax, min(r1 - tt - kTileMax, kTileMax), buf ^ 1);
+                    else claim(buf ^ 1);
+                }
+            } else {
+                long long t_n = t_i + gridDim.x;
+                if (t_n < ntiles) stage(base + t_n * tile, (int)min((long long)tile, nb - t_n * tile), buf ^ 1);
+            }
             if (buf == 0) { mbar_wait(&s_bar[0], par0); par0 ^= 1; } else { mbar_wait(&s_bar[1], par1); par1 ^= 1; }
-            const int cnt = (int)min((long long)tile, nb - t_i * tile);
+            const int cnt = UBK ? min(r1 - tt, kTileMax) : (int)min((long long)tile, nb - t_i * tile);
             const int32_t *xu = s_idx[buf][0], *xi = s_idx[buf][1], *xj = s_idx[buf][2];
             float t_loss = 0.f, t_l1u = 0.f, t_l1i = 0.f, t_l1j = 0.f, t_s2u = 0.f, t_s2i = 0.f, t_s2j = 0.f, t_gb0 = 0.f;
 
@@ -496,13 +603,20 @@ __device__ __forceinline__ void bpr_steps_body(StepParams &p, XCH &xch)
                                     if (!pw) det_red(p.ws.gQ64 + oj[r] + cc * VEC + e, gj.v[e]);
                                 }
                             } else {
-                                red_row<VEC>(p.ws.gP + ou[r] + cc * VEC, gu);
+                                if constexpr (UBK) {
+                                    float *d = s_gp + (iu[r] - u0) * (F + 1) + cc * VEC;
+#pragma unroll
+                                    for (int e = 0; e < VEC; ++e) atomicAdd(d + e, gu.v[e]);
+                                } else {
+                                    red_row<VEC>(p.ws.gP + ou[r] + cc * VEC, gu);
+                                }
                                 red_row<VEC>(p.ws.gQ + oi[r] + cc * VEC, gi);
                                 if (!pw) red_row<VEC>(p.ws.gQ + oj[r] + cc * VEC, gj);
                             }
                         }
                         if (gl == 0) {
-                            red_add_u32(p.ws.cntU + iu[r], 1u);
+                            if constexpr (UBK) atomicAdd(s_cu + (iu[r] - u0), 1u);
+                            else red_add_u32(p.ws.cntU + iu[r], 1u);
                             red_add_u64(p.ws.cntI + ii[r], 1ull);
                             if (!pw) red_add_u64(p.ws.cntI + ij[r], 1ull << 32);
                             if (GEN && p.bias != nullptr) {   // d loss / d (u_bias, i_bias, bias_): no regulariser (:76-95)
@@ -531,6 +645,21 @@ __device__ __forceinline__ void bpr_steps_body(StepParams &p, XCH &xch)
             }
             __syncthreads();  // tile buffer free for re-staging
             buf ^= 1;
+            if constexpr (UBK) {
+                tt += kTileMax;
+                if (tt >= r1) {   // the bucket is complete: one plain store per touched row and counter; untouched rows keep zeros
+                    for (int k = tid; k < rows * chunks; k += kThreads) {
+                        const int r = k / chunks, c = k - r * chunks;
+                        if (s_cu[r] == 0u) continue;
+                        const float *a = s_gp + r * (F + 1) + c * VEC;
+                        __stcg(reinterpret_cast<float4 *>(p.ws.gP + (size_t)(u0 + r) * F + c * VEC), make_float4(a[0], a[1], a[2], a[3]));
+                    }
+                    for (int k = tid; k < rows; k += kThreads)
+                        if (s_cu[k] != 0u) __stcg(p.ws.cntU + u0 + k, s_cu[k]);
+                    __syncthreads();   // accumulator free; s_claim holds the bucket claimed during this tile
+                    bk = s_claim[0]; r0 = s_claim[1]; r1 = s_claim[2]; tt = r0;
+                }
+            }
         }
         // CTA reduction of the 7 partial sums -> one fp64 atomic each
         __syncthreads();
@@ -546,6 +675,8 @@ __device__ __forceinline__ void bpr_steps_body(StepParams &p, XCH &xch)
         }
         }  // phase 1
         if (p.phases == 3) grid_barrier(&hdr->barrier, epoch);
+        if constexpr (UBK)
+            if (blockIdx.x == 0 && tid == 0) p.ub_count[2 * p.ub_buckets] = 0u;   // every claim of this step is done
         if (!(p.phases & 2)) break;   // split mode: the host reduces gQ / counters / acc across ranks now
         if (GEN && p.det) {
             // fixed-point scalar sums -> acc (the table sums stay in fixed point: the DET sweep reads and clears them)
@@ -720,11 +851,11 @@ __global__ void __launch_bounds__(kThreads, DRB_MINB) mf_bpr_steps_kernel(StepPa
     bpr_steps_body<VEC, W, NCH, GEN, NoExchange>(p, x);
 }
 
-template <int VEC, int W, int NCH>
+template <int VEC, int W, int NCH, bool UBK = false>
 __global__ void __launch_bounds__(kThreads, DRB_MINB) mf_bpr_steps_lean_kernel(StepParams p)
 {
     NoExchange x;
-    bpr_steps_body<VEC, W, NCH, false, NoExchange, true>(p, x);
+    bpr_steps_body<VEC, W, NCH, false, NoExchange, true, UBK>(p, x);
 }
 
 // the conditions under which the lean body computes what the general one does

@@ -77,12 +77,15 @@ int drb_index_range_check(const void *d_ids, int32_t elem_bytes, int64_t n_rows,
  * GeneralRecommender.fit, daisy/model/AbstractRecommender.py:112-128, for MF): returns 1 for a lean MF instantiation (its own
  * lane geometry; selected once per process on the device: every candidate geometry must reproduce the general instantiation's
  * losses and tables on a small seeded problem, the fastest one on an L2-regime timing problem is used if it beats the general
- * instantiation), 0 for the general one.  table_rows = user_num + item_num selects the regime the choice was made in: tables and
+ * instantiation), 2 for its user-bucketed mode (single-GPU fused steps of at least 524 288 triples, chosen the same way),
+ * 0 for the general one.  table_rows = user_num + item_num selects the regime the choice was made in: tables and
  * accumulators inside the L2 cache (also table_rows = 0) or streamed from HBM.  lanes / chunks (optional) receive the lanes per row and chunks of 4 floats per lane. */
 int drb_mf_step_variant(int32_t factors, int64_t table_rows, int32_t *lanes, int32_t *chunks);
 /* The timing half of that selection: milliseconds the general instantiation and the best lean candidate took for the same 3
  * steps of 524 288 triples, and the index-tile cap (512 or 1 024 triples) the chosen one runs with. */
 int drb_mf_step_selfcheck_ms(int32_t factors, int64_t table_rows, float *ms_general, float *ms_lean, int32_t *tile_cap);
+/* Which instantiation the last BPR step launch ran: 0 general, 1 lean, 2 lean user-bucketed. */
+int drb_mf_last_step_mode(void);
 /* Host-only companion (no device): lane geometry of the lean (lean != 0) or canonical instantiation, and the tile size the
  * launcher picks for `per_cta` triples per CTA and step.  DRB_ERR_INVALID when no instantiation exists for `factors`. */
 int drb_mf_step_geometry(int32_t factors, int32_t lean, int32_t *lanes, int32_t *chunks, int64_t per_cta, int32_t *tile);
