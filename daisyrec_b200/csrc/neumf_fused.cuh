@@ -523,10 +523,15 @@ template <int F>
 static int launch_neumf_fused_f(const FusedParams &p, cudaStream_t st)
 {
     using L = FusedLayout<F>;
-    static bool attr_set = false;
-    if (!attr_set) {
+    // the dynamic shared-memory limit is a per-device function attribute: remember, per calling thread, the devices it was
+    // set on (bit d for device d < 64; devices beyond set it on every launch)
+    static thread_local unsigned long long attr_set = 0ull;
+    int dev = 0;
+    DRB_CUDA(cudaGetDevice(&dev));
+    const unsigned long long bit = dev < 64 ? 1ull << dev : 0ull;
+    if (!(attr_set & bit) || bit == 0ull) {
         DRB_CUDA(cudaFuncSetAttribute(neumf_fused_kernel<F>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)L::BYTES));
-        attr_set = true;
+        attr_set |= bit;
     }
     long long tiles = (p.B + kFusedTile - 1) / kFusedTile;
     int grid = (int)(tiles < (long long)sm_count() ? tiles : (long long)sm_count());
