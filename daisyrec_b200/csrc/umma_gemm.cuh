@@ -100,12 +100,18 @@ __host__ __device__ __forceinline__ uint32_t umma_lbo(bool mn_major, int rows)
 __host__ __device__ __forceinline__ uint32_t umma_sbo(bool mn_major) { return mn_major ? 144u : 128u; }
 
 //   MN = false: src(r, k) = S[(r0 + r) * ld + k]       MN = true: src(r, k) = S[k * ld + (r0 + r)]
+// An item reads its 8 floats with two 16-byte loads only when that address is 16-byte aligned: S itself aligned, ld a multiple
+// of 4, and the item's start a multiple of 4 (k always is: chunks start at multiples of kUmmaBK; the row is checked).  Column
+// slices of a wider matrix (NGCF's T half of [S | T] at an input width that is not a multiple of 4, its W1 / W2 blocks at a
+// float offset in the parameter block that is not a multiple of 4 -- W2 starts out * (in + 1) floats after W1, odd for an
+// odd out and an even in) are staged float by float.
 template <bool MN>
 __device__ __forceinline__ void umma_stage_tile(unsigned char *smem, int rows, const float *__restrict__ S, long long ld,
                                                 long long r0, long long r_lim, int k0, int k_lim, int tid, int nthreads)
 {
     const uint32_t lbo = umma_lbo(MN, rows);
     const int items = MN ? (rows / 8) * kUmmaBK : rows * (kUmmaBK / 8);
+    const bool vec = ((reinterpret_cast<uintptr_t>(S) & 15) == 0) && ((ld & 3) == 0);
     for (int it = tid; it < items; it += nthreads) {
         float v[8];
         uint32_t off;
@@ -113,7 +119,7 @@ __device__ __forceinline__ void umma_stage_tile(unsigned char *smem, int rows, c
             const int r = it / (kUmmaBK / 8), c1 = it % (kUmmaBK / 8);    // 4 lanes read 128 contiguous bytes of a row
             const long long gr = r0 + r;
             const int k = k0 + c1 * 8;
-            if (gr < r_lim && k + 8 <= k_lim && ((ld & 3) == 0)) {
+            if (vec && gr < r_lim && k + 8 <= k_lim) {
                 const float4 *p = reinterpret_cast<const float4 *>(S + gr * ld + k);
                 float4 a = __ldg(p), b = __ldg(p + 1);
                 v[0] = a.x; v[1] = a.y; v[2] = a.z; v[3] = a.w; v[4] = b.x; v[5] = b.y; v[6] = b.z; v[7] = b.w;
@@ -126,7 +132,7 @@ __device__ __forceinline__ void umma_stage_tile(unsigned char *smem, int rows, c
             const int rg = it % (rows / 8), c = it / (rows / 8);          // consecutive lanes read consecutive row groups
             const long long gr = r0 + (long long)rg * 8;
             const int k = k0 + c;
-            if (k < k_lim && gr + 8 <= r_lim && ((ld & 3) == 0) && ((gr & 3) == 0)) {
+            if (vec && k < k_lim && gr + 8 <= r_lim && ((gr & 3) == 0)) {
                 const float4 *p = reinterpret_cast<const float4 *>(S + (long long)k * ld + gr);
                 float4 a = __ldg(p), b = __ldg(p + 1);
                 v[0] = a.x; v[1] = a.y; v[2] = a.z; v[3] = a.w; v[4] = b.x; v[5] = b.y; v[6] = b.z; v[7] = b.w;
