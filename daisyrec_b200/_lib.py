@@ -152,6 +152,15 @@ SIGNATURES = {
     "drb_sampler_draw_mt19937_mixed": (C.c_int, [vp, vp, C.c_int32, C.c_int32, C.c_int32, C.c_int32, vp, vp, c_i32p]),
     "drb_sampler_assemble_mixed": (C.c_int, [vp, vp, vp, vp, vp, C.c_int32, C.c_int32, C.c_int32, C.c_int32, vp, vp]),
     "drb_sampler_explode_pointwise": (C.c_int, [vp, vp, vp, C.c_int64, vp, C.c_int32, vp, vp]),
+    "drb_skipgram_workspace_bytes": (C.c_size_t, [C.c_int32, C.c_int64]),
+    "drb_skipgram_group": (C.c_int, [vp, C.c_int64, C.c_int32, C.c_int32, vp, vp, vp, vp, vp]),
+    "drb_skipgram_draws_mt19937": (C.c_int, [vp, vp, vp, C.c_int32, C.c_int32, vp, c_i32p]),
+    "drb_skipgram_emit": (C.c_int, [vp, vp, vp, C.c_int64, C.c_int32, vp, vp, vp, vp, vp, vp, vp]),
+    "drb_i2v_workspace_bytes": (C.c_size_t, [C.c_int32, C.c_int32, C.c_int32]),
+    "drb_i2v_workspace_init": (C.c_int, [vp, C.c_int32, C.c_int32, C.c_int32, vp]),
+    "drb_i2v_train_steps": (C.c_int, [vp, vp, C.c_int32, C.c_int32, vp, vp, vp, C.c_int64, C.c_int64, C.c_int64, C.c_int64,
+                                      C.POINTER(Hyper), C.c_int64, C.c_int32, vp, C.c_int32, c_i64p, vp]),
+    "drb_i2v_user_embedding": (C.c_int, [vp, C.c_int32, vp, vp, C.c_int32, vp, vp]),
     "drb_csr_workspace_bytes": (C.c_size_t, [C.c_int32, C.c_int64]),
     "drb_csr_build": (C.c_int, [vp, vp, C.c_int64, C.c_int32, C.c_int32, vp, vp, vp, c_i64p, vp]),
     "drb_lgcn_build_adj": (C.c_int, [vp, vp, vp, vp, C.c_int32, C.c_int32, C.c_int64, vp, vp, vp, vp]),

@@ -305,6 +305,31 @@ extern "C" int drb_bounded_draws_mt19937(uint32_t *st, const int64_t *h_n, const
     return DRB_OK;
 }
 
+// Skip-gram negatives (daisy/utils/sampler.py:136-158): users ascending, every position i of a sequence of length L draws
+// c_i = min(L-1, i+w) - max(0, i-w) ranks from [0, n[u]) -- the order of the reference's np.random.choice calls, and the order
+// drb_skipgram_emit reads them in.  Users without a sequence draw nothing; an empty complement fails only if it is drawn from.
+extern "C" int drb_skipgram_draws_mt19937(uint32_t *st, const int64_t *h_n, const int64_t *h_seq_len, int32_t U, int32_t window,
+                                          int32_t *h_draws, int32_t *bad_user)
+{
+    DRB_REQUIRE(st && h_n && h_seq_len && U >= 0 && window >= 0, "skipgram_draws_mt19937: bad arguments");
+    Mt mt{st, st + 624};
+    int64_t d = 0;
+    for (int32_t u = 0; u < U; ++u) {
+        const int64_t L = h_seq_len[u];
+        for (int64_t i = 0; i < L; ++i) {
+            const int64_t lo = i - window > 0 ? i - window : 0, hi = i + window < L - 1 ? i + window : L - 1;
+            const int64_t c = hi - lo;
+            if (c > 0 && h_n[u] <= 0) {
+                if (bad_user) *bad_user = u;
+                set_error("'a' cannot be empty: user %d has interacted with every item", u);
+                return DRB_ERR_EMPTY_SET;
+            }
+            for (int64_t m = 0; m < c; ++m) h_draws[d++] = (int32_t)mt.bounded((uint32_t)h_n[u]);
+        }
+    }
+    return DRB_OK;
+}
+
 extern "C" int drb_kth_complement_var(const int64_t *d_row_ptr, const int32_t *d_col, const int64_t *d_offsets,
                                       const int32_t *d_draws, int64_t rows, int32_t *d_out, void *stream)
 {

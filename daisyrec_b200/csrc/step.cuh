@@ -76,6 +76,8 @@ struct StepParams {
     Workspace ws = {};
     const int32_t *bu = nullptr, *bi = nullptr, *bj = nullptr;
     long long n = 0, batch = 0, first_step = 0, n_steps = 0;
+    // U = 0 (GEN only): Item2Vec's one tied table.  The launcher sets P = Q and gP = gQ, so both operands gather from and
+    // accumulate into the item table, the first operand's occurrence is counted in cntI and phase 2 sweeps the item table alone.
     int U = 0, I = 0, F = 0, tile = 0;   // tile: set by the launcher before every launch
     float lr = 0.f, reg1 = 0.f, reg2 = 0.f;
     int opt = DRB_OPT_SGD;

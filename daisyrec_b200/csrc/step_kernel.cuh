@@ -616,6 +616,7 @@ __device__ __forceinline__ void bpr_steps_body(StepParams &p, XCH &xch)
                         }
                         if (gl == 0) {
                             if constexpr (UBK) atomicAdd(s_cu + (iu[r] - u0), 1u);
+                            else if (GEN && p.U == 0) red_add_u64(p.ws.cntI + iu[r], 1ull);
                             else red_add_u32(p.ws.cntU + iu[r], 1u);
                             red_add_u64(p.ws.cntI + ii[r], 1ull);
                             if (!pw) red_add_u64(p.ws.cntI + ij[r], 1ull << 32);

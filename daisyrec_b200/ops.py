@@ -198,6 +198,42 @@ def sampler_explode_pointwise(d_coo_u, d_coo_i, d_label, d_js):
 
 
 # ------------------------------------------------------------------ CSR / adjacency builders
+def skipgram_group(d_coo_u, user_num, window):
+    """Device: (seq_ptr int64 [U+1], ctx_ptr int64 [U+1], order int32 [nnz]) -- the train rows grouped by user in row order."""
+    _dev(d_coo_u, torch.int32, "coo_u")
+    n, dev = d_coo_u.numel(), d_coo_u.device
+    ws = torch.empty(max(1, L.lib().drb_skipgram_workspace_bytes(user_num, n)), dtype=torch.uint8, device=dev)
+    seq_ptr = torch.empty(user_num + 1, dtype=torch.int64, device=dev)
+    ctx_ptr = torch.empty(user_num + 1, dtype=torch.int64, device=dev)
+    order = torch.empty(max(1, n), dtype=torch.int32, device=dev)
+    L.check(L.lib().drb_skipgram_group(_ptr(d_coo_u), n, user_num, window, _ptr(ws), _ptr(seq_ptr), _ptr(ctx_ptr),
+                                       _ptr(order), _stream()))
+    return seq_ptr, ctx_ptr, order[:n]
+
+
+def skipgram_draws_mt19937(state, n, seq_len, window, total):
+    """Host: the ``total`` negative ranks of the skip-gram sampler off numpy's MT19937 stream (advances ``state``)."""
+    n = np.ascontiguousarray(n, np.int64)
+    seq_len = np.ascontiguousarray(seq_len, np.int64)
+    draws = np.empty(max(1, total), np.int32)
+    bad = C.c_int32(-1)
+    L.check(L.lib().drb_skipgram_draws_mt19937(state.ctypes.data, n.ctypes.data, seq_len.ctypes.data, len(n), window,
+                                               draws.ctypes.data, C.byref(bad)))
+    return draws[:total]
+
+
+def skipgram_emit(d_coo_u, d_coo_i, d_order, window, d_seq_ptr, d_ctx_ptr, d_row_ptr, d_col, d_draws, total):
+    """Device: int32 [2 * total, 3] skip-gram rows."""
+    for t, nm in ((d_coo_u, "coo_u"), (d_coo_i, "coo_i"), (d_order, "order"), (d_col, "col"), (d_draws, "draws")):
+        _dev(t, torch.int32, nm)
+    for t, nm in ((d_seq_ptr, "seq_ptr"), (d_ctx_ptr, "ctx_ptr"), (d_row_ptr, "row_ptr")):
+        _dev(t, torch.int64, nm)
+    rows = torch.empty((2 * total, 3), dtype=torch.int32, device=d_coo_u.device)
+    L.check(L.lib().drb_skipgram_emit(_ptr(d_coo_u), _ptr(d_coo_i), _ptr(d_order), d_order.numel(), window, _ptr(d_seq_ptr),
+                                      _ptr(d_ctx_ptr), _ptr(d_row_ptr), _ptr(d_col), _ptr(d_draws), _ptr(rows), _stream()))
+    return rows
+
+
 def csr_build(d_row, d_col, n_rows, n_cols):
     """COO int32 pairs on the device -> (row_ptr int64[n_rows+1], col int32[nnz_unique]) sorted + duplicate-free."""
     _dev(d_row, torch.int32, "row"); _dev(d_col, torch.int32, "col")
@@ -388,6 +424,38 @@ def mf_bpr_train_steps_host(P, Q, ws, h_bu, h_bi, h_bj, batch, n_steps, hp, adam
                                              _ptr(stage), _ptr(d_loss), h_loss.data_ptr(), C.byref(nan_step), _stream())
     L.check(rc)
     return h_loss[:n_steps]
+
+
+# ------------------------------------------------------------------ Item2Vec
+class I2VWorkspace:
+    """Step-kernel scratch of the one tied item table: gradient accumulator, row counters, Adam m and v."""
+
+    def __init__(self, item_num, factors, opt, device):
+        self.I, self.F = item_num, factors
+        self.opt = L.OPT_KIND[opt]
+        self.buf = torch.empty(L.lib().drb_i2v_workspace_bytes(item_num, factors, self.opt), dtype=torch.uint8, device=device)
+        L.check(L.lib().drb_i2v_workspace_init(_ptr(self.buf), item_num, factors, self.opt, _stream()))
+
+
+def i2v_train_steps(Q, ws, bt, bc, blabel, batch, first_step, n_steps, hp, adam_step0=0, apply=True, check=True):
+    """Skip-gram steps on (target, context, label) planes; float64 device losses [n_steps].  apply=False: loss of one batch."""
+    _dev(Q, torch.float32, "Q")
+    for t, nm in ((bt, "target"), (bc, "context"), (blabel, "label")):
+        _dev(t, torch.int32, nm)
+    losses = torch.empty(max(n_steps, 1), dtype=torch.float64, device=Q.device)
+    nan_step = C.c_int64(-1)
+    L.check(L.lib().drb_i2v_train_steps(_ptr(Q), _ptr(ws.buf), ws.I, ws.F, _ptr(bt), _ptr(bc), _ptr(blabel), bt.numel(), batch,
+                                        first_step, n_steps, C.byref(hp), adam_step0, 1 if apply else 0, _ptr(losses),
+                                        1 if check else 0, C.byref(nan_step), _stream()))
+    return losses[:n_steps]
+
+
+def i2v_user_embedding(Q, d_row_ptr, d_col, P):
+    """P[u] = sum of Q over the user's CSR row, for the users with a non-empty row (in place)."""
+    _dev(Q, torch.float32, "Q"); _dev(P, torch.float32, "P")
+    _dev(d_row_ptr, torch.int64, "row_ptr"); _dev(d_col, torch.int32, "col")
+    L.check(L.lib().drb_i2v_user_embedding(_ptr(Q), Q.shape[1], _ptr(d_row_ptr), _ptr(d_col), P.shape[0], _ptr(P), _stream()))
+    return P
 
 
 # ------------------------------------------------------------------ FM

@@ -27,7 +27,8 @@ def fingerprint(a):
 
 
 class TripleArray(np.ndarray):
-    """int32 [T,3] host array that remembers its device twin (saves fit() a 12*T-byte H2D).  Views / copies forget
+    """[T,3] host array (int32, or the skip-gram sampler's int64) that remembers its int32 device twin (saves fit() a
+    12*T-byte H2D).  Views / copies forget
     the twin; an in-place edit is caught by the stamp taken when the twin was attached."""
     _drb_device = None
     _drb_stamp = None
@@ -147,3 +148,48 @@ class BasicNegtiveSampler(AbstractSampler):
             return self._pointwise(torch.from_numpy(coo_u).cuda(), torch.from_numpy(coo_i).cuda(), d_js)
         d_tr = ops.sampler_explode(torch.from_numpy(coo_u).cuda(), torch.from_numpy(coo_i).cuda(), d_js)
         return TripleArray.attach(d_tr.cpu().numpy(), d_tr)
+
+
+class SkipGramNegativeSampler(AbstractSampler):
+    """Skip-gram rows of Item2Vec (daisy/utils/sampler.py:105-160), computed on the device through the C ABI.
+
+    Sequences are the rows of ``df`` grouped by user (users ascending, row order, duplicates kept).  Position i of a sequence
+    yields (target, context, 1) for every context within ``context_window`` positions, then as many (target, negative, 0)
+    rows, the negatives drawn like np.random.choice(setdiff1d(arange(item_num), train_ur[u])) off numpy's global stream,
+    which is advanced exactly as the reference advances it.  ``discard=True`` first drops each row with probability
+    1 - sqrt(rho / count(item)), drawing np.random.uniform(size=len(df)) as the reference does.
+    """
+
+    def __init__(self, df, config, discard=False):
+        super().__init__(config)
+        self.context_window = config['context_window']
+        self.user_num = config.get('user_num')
+        self.csr = config.get('train_csr', None)                   # (row_ptr int64, col int32) to skip the dict walk
+        if discard:                                                # sampler.py:125-131
+            items = df[self.iid_name]
+            prob_discard = 1 - np.sqrt(config['rho'] / items.value_counts())
+            rnd_p = np.random.uniform(low=0., high=1., size=len(df))
+            df = df[rnd_p >= items.map(prob_discard).values]
+        self.coo_u = np.array(df[self.uid_name].values, dtype=np.int32)
+        self.coo_i = np.array(df[self.iid_name].values, dtype=np.int32)
+        if self.user_num is None:
+            self.user_num = 1 + max(int(self.coo_u.max(initial=-1)), max(self.ur.keys(), default=-1))
+
+    def sampling(self):
+        """-> int64 [T, 3] host rows (the reference's array) carrying their int32 device twin."""
+        ops.require_cuda()
+        U, I, w = int(self.user_num), int(self.item_num), int(self.context_window)
+        row_ptr, col = self.csr if self.csr is not None else csr_from_ur(self.ur, U)
+        d_u = torch.from_numpy(self.coo_u).cuda()
+        d_i = torch.from_numpy(self.coo_i).cuda()
+        seq_ptr, ctx_ptr, order = ops.skipgram_group(d_u, U, w)
+        seq_len = np.diff(seq_ptr.cpu().numpy())
+        total = int(ctx_ptr[-1].item())
+        state = ops.mt19937_from_numpy()
+        draws = ops.skipgram_draws_mt19937(state, I - np.diff(np.asarray(row_ptr, np.int64)), seq_len, w, total)
+        ops.mt19937_to_numpy(state)                                # numpy's stream moves on as in the reference
+        d_rows = ops.skipgram_emit(d_u, d_i, order, w, seq_ptr, ctx_ptr,
+                                   torch.from_numpy(np.ascontiguousarray(row_ptr, np.int64)).cuda(),
+                                   torch.from_numpy(np.ascontiguousarray(col, np.int32)).cuda(),
+                                   torch.from_numpy(draws).cuda(), total)
+        return TripleArray.attach(d_rows.cpu().numpy().astype(np.int64), d_rows)

@@ -131,6 +131,40 @@ int drb_sampler_assemble_mixed(const int64_t *d_row_ptr, const int32_t *d_col, c
 int drb_sampler_explode_pointwise(const int32_t *d_coo_u, const int32_t *d_coo_i, const int32_t *d_label, int64_t nnz,
                                   const int32_t *d_js, int32_t num_ng, int32_t *d_rows, void *stream);
 
+/* ---- skip-gram sampler: SkipGramNegativeSampler.sampling() (daisy/utils/sampler.py:105-160) ----------
+ * Sequences = the train rows grouped by user (users ascending, row order kept, duplicates kept).  Position i of a
+ * sequence of length L has c_i = min(L-1, i+w) - max(0, i-w) contexts; it yields c_i rows (target, context, 1) in context
+ * order, then c_i rows (target, neg, 0), neg drawn uniformly from the items outside the user's train row.  T = 2 sum c_i.
+ * drb_skipgram_group          device: d_seq_ptr [U+1] = sequence offsets, d_ctx_ptr [U+1] = offsets of the users' draws
+ *                             (d_ctx_ptr[U] = sum c_i), d_order [nnz] = row ids grouped by user in row order.
+ *                             DRB_ERR_INVALID if a user id lies outside [0, user_num).  Synchronises the stream.
+ * drb_skipgram_draws_mt19937  host: the sum c_i bounded draws off numpy's MT19937 stream, h_n[u] = item_num - |train_ur[u]|,
+ *                             h_seq_len[u] = sequence length; DRB_ERR_EMPTY_SET if a user with contexts has no complement.
+ * drb_skipgram_emit           device: int32 [T, 3] rows; each negative = the draw-th item outside the user's sorted CSR row. */
+size_t drb_skipgram_workspace_bytes(int32_t user_num, int64_t nnz);
+int drb_skipgram_group(const int32_t *d_coo_u, int64_t nnz, int32_t user_num, int32_t window, void *d_ws, int64_t *d_seq_ptr,
+                       int64_t *d_ctx_ptr, int32_t *d_order, void *stream);
+int drb_skipgram_draws_mt19937(uint32_t *h_state625, const int64_t *h_n, const int64_t *h_seq_len, int32_t user_num,
+                               int32_t window, int32_t *h_draws, int32_t *bad_user);
+int drb_skipgram_emit(const int32_t *d_coo_u, const int32_t *d_coo_i, const int32_t *d_order, int64_t nnz, int32_t window,
+                      const int64_t *d_seq_ptr, const int64_t *d_ctx_ptr, const int64_t *d_row_ptr, const int32_t *d_col,
+                      const int32_t *d_draws, int32_t *d_rows, void *stream);
+
+/* ---- Item2Vec: Item2Vec.fit / calc_loss (daisy/model/Item2VecRecommender.py:16-107) ---------------------
+ * One tied fp32 table Q [item_num, factors] (shared_embedding.weight).  drb_i2v_train_steps = the persistent step of
+ * drb_mf_bpr_train_steps with loss CL on (target, context, label) rows, both rows read from and updated in Q, no
+ * regulariser (hyper->reg_1 and reg_2 must be 0), SGD or dense Adam; apply = 0: the loss of ONE batch, no update
+ * (calc_loss).  DRB_ERR_NAN_LOSS as drb_mf_bpr_train_steps.  drb_i2v_user_embedding: P[u] = sum of Q[col[k]] over
+ * the user's CSR row, for every user with a non-empty row; the other rows of P are left as they are. */
+size_t drb_i2v_workspace_bytes(int32_t item_num, int32_t factors, int32_t opt);
+int drb_i2v_workspace_init(void *d_ws, int32_t item_num, int32_t factors, int32_t opt, void *stream);
+int drb_i2v_train_steps(float *d_Q, void *d_ws, int32_t item_num, int32_t factors, const int32_t *d_bt, const int32_t *d_bc,
+                        const int32_t *d_blabel, int64_t n, int64_t batch, int64_t first_step, int64_t n_steps,
+                        const drb_hyper *hyper, int64_t adam_step0, int32_t apply, double *d_step_loss, int32_t sync_and_check,
+                        int64_t *nan_step, void *stream);
+int drb_i2v_user_embedding(const float *d_Q, int32_t factors, const int64_t *d_row_ptr, const int32_t *d_col, int32_t user_num,
+                           float *d_P, void *stream);
+
 /* ---- candidate sets for ranking: build_candidates_set ------------------------------------
  * daisy/utils/utils.py:53-85.  Per test user the reference draws cand_num-|gt| ids from the
  * complement of gt + train positives (or, when |gt| >= cand_num, cand_num ids from gt itself).
