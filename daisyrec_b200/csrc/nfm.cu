@@ -549,6 +549,11 @@ extern "C" int drb_nfm_bpr_train_steps_dropout(float *d_P, float *d_Q, float *d_
     DRB_REQUIRE(h->opt == DRB_OPT_SGD || h->opt == DRB_OPT_ADAM, "nfm: SGD and Adam only (optimizer id %d)", h->opt);
     DRB_REQUIRE(h->loss == DRB_LOSS_BPR, "nfm: BPR only");
     if (n_steps == 0) return DRB_OK;
+    // BatchNorm1d in train mode rejects a forward call of one row (torch raises ValueError); each call here is one half of a
+    // step.  Only the last step can be short, so checking it before the first launch refuses the call with nothing changed.
+    const int64_t last_base = (first_step + n_steps - 1) * batch, last_rows = n - last_base < batch ? n - last_base : batch;
+    DRB_REQUIRE(!batch_norm || last_rows >= 2, "Expected more than 1 value per channel when training, got input size [%lld, %d]",
+                (long long)last_rows, F);
     cudaStream_t st = (cudaStream_t)stream;
     NfmWs w;
     carve_nfm(d_ws, d, h->opt, max_rows, &w);

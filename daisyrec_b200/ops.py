@@ -722,6 +722,10 @@ def nfm_bpr_train_steps(P, Q, bias, N, Rs, ws, act, bu, bi, bj, batch, first_ste
         ws.Ln, ws.bn, act, ws.max_rows, _ptr(bu), _ptr(bi), _ptr(bj), bu.numel(), batch, first_step, n_steps, C.byref(hp), adam_step0,
         1 if apply else 0, tower_dtype, None if keep is None else _ptr(keep), C.c_float(dropout if keep is not None else 0.0),
         _ptr(losses), 1 if check else 0, C.byref(nan_step), _stream())
+    if rc == L.DRB_ERR_INVALID:
+        msg = (L.lib().drb_last_error() or b"").decode(errors="replace")
+        if msg.startswith("Expected more than 1 value per channel"):      # BatchNorm1d's own ValueError in the reference
+            raise ValueError(msg)
     L.check(rc)
     return losses[:n_steps]
 
