@@ -9,6 +9,7 @@ the epoch's permutation is produced with the DataLoader's own RNG protocol (so b
 reference's batches), gathered into SoA index planes on the device, and consumed by
 ``drb_mf_bpr_train_steps``.
 """
+import functools
 import os
 
 import numpy as np
@@ -164,7 +165,34 @@ class AbstractRecommender(object):
         raise NotImplementedError(f'Invalid loss type: {self.loss_type}...')
 
 
+def packed_bias(user_num, item_num, device):
+    """FM's first-order terms as ONE device vector [u_bias (U), i_bias (I), bias_ (1)], zeroed as the reference's _init_weight
+    leaves them -> (vector, u_bias table, i_bias table, bias_ view); the three are views of the vector."""
+    bias = torch.zeros(user_num + item_num + 1, dtype=torch.float32, device=device)
+    return (bias, _Table(bias[:user_num].view(user_num, 1)), _Table(bias[user_num:user_num + item_num].view(item_num, 1)),
+            bias[user_num + item_num:])
+
+
+def ragged_split(n, batch, first, n_steps):
+    """Steps [first, first + n_steps) over n rows in batches of ``batch`` -> (full, last): ``full`` steps of whole batches, then,
+    when the last of them is ragged, one step of ``last`` rows (else last = 0).  Host-drawn dropout masks are sized per step,
+    so the ragged batch gets its own masks and launch."""
+    full = n_steps if (first + n_steps) * batch <= n else n_steps - 1
+    return full, (n - (first + full) * batch if full < n_steps else 0)
+
+
 class GeneralRecommender(AbstractRecommender):
+    """Shared plumbing of the GPU-path models.  A subclass declares its defaults and state as class data, builds its tables in
+    ``__init__`` and supplies ``_workspace(opt, rows)`` and ``_launch(bu, bi, bj, batch, first, n_steps, apply)``."""
+    DEFAULT_OPTIMIZER = 'sgd'                   # config['optimizer'] == 'default'
+    DEFAULT_INIT = 'normal'                     # config['init_method'] == 'default'
+    MULTI_GPU = '{} runs as independent replicas only (DESIGN.md, multi-GPU section)'   # None: the class shards under torchrun
+    LOSS_TYPE = None                            # a fixed, unregularised loss: loss_type, reg_1 and reg_2 are not read
+    PARAMS = ('embed_user.weight', 'embed_item.weight')     # parameters() in order; attribute paths
+    BUFFERS = ()                                # in state_dict() after PARAMS, not in parameters()
+    STRICT_STATE = True                         # load_state_dict: every key of state_dict() must be given
+    SCRATCH_KEY = None                          # config key of the row count of a batch-sized scratch (built at first step)
+
     def __init__(self, config):
         super().__init__()
         gpu = str(config.get('gpu', '') or '')
@@ -184,6 +212,180 @@ class GeneralRecommender(AbstractRecommender):
         import torch.distributed as dist
         self.world = dist.get_world_size() if dist.is_available() and dist.is_initialized() else 1
         self.rank_id = dist.get_rank() if self.world > 1 else 0
+        if self.world > 1 and self.MULTI_GPU is not None:
+            raise NotImplementedError(self.MULTI_GPU.format(type(self).__name__))
+        # the reference's common keys (e.g. MFRecommender.py:46-59)
+        self.lr, self.epochs, self.topk = config['lr'], config['epochs'], config['topk']
+        self.user_num, self.item_num, self.factors = config['user_num'], config['item_num'], config['factors']
+        if self.LOSS_TYPE is None:
+            self.loss_type, self.reg_1, self.reg_2 = config['loss_type'], config['reg_1'], config['reg_2']
+        else:
+            self.loss_type, self.reg_1, self.reg_2 = self.LOSS_TYPE, 0., 0.
+        self.optimizer = config['optimizer'] if config['optimizer'] != 'default' else self.DEFAULT_OPTIMIZER
+        self.initializer = config['init_method'] if config['init_method'] != 'default' else self.DEFAULT_INIT
+        self.early_stop = config['early_stop']
+        if self.SCRATCH_KEY is not None:
+            self._rows = int(config.get(self.SCRATCH_KEY, 1 << 16))
+        self._hp = self._ws = None
+        self._opt_steps = 0
+
+    # ------------------------------------------------------------------ state
+    def state_dict(self):
+        return {k: functools.reduce(getattr, k.split('.'), self) for k in self.PARAMS + self.BUFFERS}
+
+    def parameters(self):
+        sd = self.state_dict()
+        return [sd[k] for k in self.PARAMS]
+
+    def load_state_dict(self, sd):
+        for k, t in self.state_dict().items():
+            if self.STRICT_STATE or k in sd:
+                t.copy_(torch.as_tensor(sd[k]).reshape(t.shape))
+        self._drop_cache()
+
+    def _drop_cache(self):
+        """Forget whatever was computed from the parameters (the graph models' propagated tables)."""
+
+    def to(self, device):
+        return self
+
+    # ------------------------------------------------------------------ steps
+    def _hyper(self, opt=None):
+        opt = opt or self._optimizer_name()
+        if self.SUPPORTED_LOSSES == ('BPR',):                     # the BPR-only steps take the default loss kind
+            return ops.hyper(self.lr, self.reg_1, self.reg_2, opt)
+        return ops.hyper(self.lr, self.reg_1, self.reg_2, opt, loss=str(self.loss_type).upper())
+
+    def _begin_fit(self, opt):
+        """fit() builds a fresh optimizer (AbstractRecommender.py:105): fresh optimiser state and step count.  A batch-sized
+        scratch waits for the first step, which knows the batch size."""
+        self._hp = self._hyper(opt)
+        self._opt_steps = 0
+        self._fit_opt = opt
+        self._ws = None if self.SCRATCH_KEY is not None else self._workspace(opt)
+
+    def _ensure(self, rows=0):
+        """Optimiser state and scratch for a step of ``rows`` scratch rows; a step outside fit() starts a fresh optimiser."""
+        if self._hp is None:
+            self._begin_fit(self._optimizer_name())
+        if self.SCRATCH_KEY is None:
+            return
+        rows = max(int(rows), self._rows)
+        if self._ws is None:
+            self._ws = self._workspace(self._fit_opt, rows)
+        elif self._ws.max_rows < rows:
+            # growing the scratch would drop the optimiser state: size it up front instead
+            raise RuntimeError(f'{type(self).__name__} scratch too small; set config["{self.SCRATCH_KEY}"] >= 2 * batch_size')
+
+    def _train_steps(self, bu, bi, bj, batch, first, n_steps):
+        self._ensure(2 * batch)
+        losses = self._launch(bu, bi, bj, batch, first, n_steps, apply=True)
+        self._opt_steps += n_steps
+        return losses
+
+    def calc_loss(self, batch):
+        """0-d fp32 loss of one (user, pos, neg) -- or (user, item, label) -- batch; no update."""
+        self._check_loss_type()
+        bu, bi, bj = self._batch_ids(batch)
+        self._ensure(2 * bu.numel())
+        return self._launch(bu, bi, bj, bu.numel(), 0, 1, apply=False).to(torch.float32).reshape(())
+
+    def train_step(self, batch):
+        """zero_grad + calc_loss + backward + optimizer.step on one batch, in train mode (AbstractRecommender.py:119-128)
+        -> loss.item()."""
+        self._check_loss_type()
+        bu, bi, bj = self._batch_ids(batch)
+        self._ensure(2 * bu.numel())
+        was = self.training
+        self.train()
+        try:
+            return float(self._train_steps(bu, bi, bj, bu.numel(), 0, 1).item())
+        finally:
+            self.train(was)
+
+    # ------------------------------------------------------------------ caller ids
+    def _check_ids(self, cols, bounds, names):
+        """nn.Embedding's IndexError when a column of caller ids leaves [0, bounds[c]): the kernels index raw tables.  Host
+        columns are checked on the host (no device sync), device columns in one ops.check_index_range launch."""
+        dev = []
+        for ids, hi, what in zip(cols, bounds, names):
+            t = torch.as_tensor(ids)
+            if t.is_cuda:
+                dev.append((t.reshape(-1).to(torch.int64), hi, what))
+            elif t.numel():
+                h = t.reshape(-1).to(torch.int64)
+                bad = int(((h < 0) | (h >= hi)).sum())
+                if bad:
+                    raise IndexError(f"index out of range in self: {bad} {what} id(s) outside [0, {int(hi)})")
+        if dev:
+            ids, bounds, names = zip(*dev)
+            ops.check_index_range(torch.stack(ids, 1).contiguous(), bounds, names)
+
+    def _device_ids(self, cols, bounds, names, dtype=torch.int32):
+        """Range-checked caller ids -> one contiguous 1-D device tensor of ``dtype`` per column."""
+        self._check_ids(cols, bounds, names)
+        return [torch.as_tensor(c).to(self.device, dtype).reshape(-1).contiguous() for c in cols]
+
+    def _batch_ids(self, batch):
+        return self._device_ids(batch[:3], *self._index_bounds())
+
+    def _pair_ids(self, user, item, dtype=torch.int32):
+        return self._device_ids((user, item), (self.user_num, self.item_num), ('user', 'item'), dtype)
+
+    # ------------------------------------------------------------------ ranking
+    def _rank_inputs(self, test_loader):
+        """The test loader's (users int64 [n], candidates int64 [n, C], topk) on the host, range-checked; None when it is
+        empty.  Reads ``dataset.data`` of a CandidatesDataset loader in bulk, else iterates (us, cands_ids) batches."""
+        data = getattr(getattr(test_loader, 'dataset', None), 'data', None)
+        if isinstance(data, (list, tuple)) and len(data) and len(data[0]) == 2:
+            users = np.fromiter((int(r[0]) for r in data), np.int64, len(data))
+            cands = np.stack([np.asarray(r[1], dtype=np.int64) for r in data])
+        else:
+            us, cs = [], []
+            for b_us, b_c in test_loader:
+                us.append(torch.as_tensor(b_us).reshape(-1).to(torch.int64))
+                cs.append(torch.as_tensor(b_c).to(torch.int64).reshape(us[-1].numel(), -1))
+            if not us:
+                return None
+            users, cands = torch.cat(us).numpy(), torch.cat(cs).numpy()
+        if len(users) == 0:
+            return None
+        self._check_ids((users, cands), (self.user_num, self.item_num), ('test user', 'candidate item'))
+        return users, np.ascontiguousarray(cands), min(self.topk, cands.shape[1])
+
+    def _dot_tables(self):
+        """(P, Q) of the dot-product scorers (MF's rank kernels)."""
+        return self.embed_user.weight, self.embed_item.weight
+
+    def _pair_scores(self, user, item):
+        """pred = (P[user] * Q[item]).sum(-1) for index tensors (MFRecommender.py:63-68)."""
+        u, i = self._pair_ids(user, item)
+        return ops.mf_predict(*self._dot_tables(), u, i)
+
+    def forward(self, user, item):
+        return self._pair_scores(user, item)
+
+    def __call__(self, *args):
+        return self.forward(*args)
+
+    def predict(self, u, i):
+        """-> python float (MFRecommender.py:99-104)."""
+        return float(self._pair_scores([u], [i]).item())
+
+    def rank(self, test_loader):
+        """-> float32 ndarray [n_test_users, topk] of the top candidates, rows in loader order (MFRecommender.py:106-123)."""
+        P, Q = self._dot_tables()
+        ins = self._rank_inputs(test_loader)
+        if ins is None:
+            return np.zeros((0,), np.float32)
+        users, cands, k = ins
+        return ops.mf_rank(P, Q, torch.from_numpy(users).to(self.device), torch.from_numpy(cands).to(self.device), k).cpu().numpy()
+
+    def full_rank(self, u):
+        """-> int64 ndarray [topk] of the top items of user u; no masking of train items (MFRecommender.py:126-133)."""
+        P, Q = self._dot_tables()
+        users = self._device_ids(([int(u)],), (self.user_num,), ('user',), torch.int64)[0]
+        return ops.mf_full_rank(P, Q, users, min(self.topk, self.item_num))[0].cpu().numpy()
 
     def _loader_plan(self, train_loader):
         return loader_plan(train_loader)

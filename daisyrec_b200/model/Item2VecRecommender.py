@@ -20,22 +20,15 @@ from .MFRecommender import MF
 
 class Item2Vec(GeneralRecommender):
     SUPPORTED_LOSSES = ('CL',)
+    DEFAULT_OPTIMIZER = 'adam'
+    LOSS_TYPE = 'CL'
+    PARAMS = ('user_embedding.weight', 'shared_embedding.weight')
 
     def __init__(self, config):
         """Same keys as the reference (Item2VecRecommender.py:18-46): user_num, item_num, factors, train_ur, lr, epochs,
         optimizer, init_method, early_stop, topk (+ gpu, logger).  loss_type is always CL."""
         super().__init__(config)
-        if self.world > 1:
-            raise NotImplementedError('Item2Vec runs as independent replicas only (DESIGN.md, multi-GPU section)')
-        self.user_num, self.item_num, self.factors = config['user_num'], config['item_num'], config['factors']
         self.ur = config['train_ur']
-        self.lr = config['lr']
-        self.epochs = config['epochs']
-        self.loss_type = 'CL'
-        self.optimizer = config['optimizer'] if config['optimizer'] != 'default' else 'adam'
-        self.initializer = config['init_method'] if config['init_method'] != 'default' else 'normal'
-        self.early_stop = config['early_stop']
-        self.topk = config['topk']
         # the reference's CPU RNG consumption: nn.Embedding(user_num), nn.Embedding(item_num), then apply(_init_weight)
         wu = _init_table(self.user_num, self.factors, None)
         wi = _init_table(self.item_num, self.factors, None)
@@ -45,58 +38,22 @@ class Item2Vec(GeneralRecommender):
         self.shared_embedding = _Table(wi.to(self.device))
         self._train_csr = config.get('train_csr', None)            # (row_ptr int64, col int32) to skip the dict walk
         self._csr_dev = None
-        self._ws = None
-        self._opt_steps = 0
 
     # MF's scoring with P = user_embedding, Q = shared_embedding (Item2VecRecommender.py:71-107 are MFRecommender.py:99-133)
     embed_user = property(lambda self: self.user_embedding)
     embed_item = property(lambda self: self.shared_embedding)
     _full_user_table = MF._full_user_table
-    forward = MF.forward
-    __call__ = MF.forward
-    predict = MF.predict
-    rank = MF.rank
-    full_rank = MF.full_rank
     full_rank_users = MF.full_rank_users
-
-    # ------------------------------------------------------------------ plumbing
-    def parameters(self):
-        return [self.user_embedding.weight, self.shared_embedding.weight]
-
-    def state_dict(self):
-        return {'user_embedding.weight': self.user_embedding.weight, 'shared_embedding.weight': self.shared_embedding.weight}
-
-    def load_state_dict(self, sd):
-        self.user_embedding.weight.copy_(sd['user_embedding.weight'])
-        self.shared_embedding.weight.copy_(sd['shared_embedding.weight'])
-
-    def to(self, device):
-        return self
 
     def _index_bounds(self):
         return (self.item_num, self.item_num, 1 << 62), ('target item', 'context item', 'label')
 
-    def _begin_fit(self, opt):
-        """A fresh optimiser per fit() (AbstractRecommender.py:105): fresh Adam moments and step count."""
-        self._hp = ops.hyper(self.lr, 0., 0., opt, loss='CL')
-        self._opt_steps = 0
-        self._ws = ops.I2VWorkspace(self.item_num, self.factors, opt, self.device)
+    def _workspace(self, opt, rows=None):
+        return ops.I2VWorkspace(self.item_num, self.factors, opt, self.device)
 
-    def _ensure_ws(self):
-        if self._ws is None:
-            self._begin_fit(self._optimizer_name())
-
-    def _train_steps(self, bu, bi, bj, batch, first, n_steps):
-        losses = ops.i2v_train_steps(self.shared_embedding.weight, self._ws, bu, bi, bj, batch, first, n_steps, self._hp,
-                                     adam_step0=self._opt_steps)
-        self._opt_steps += n_steps
-        return losses
-
-    def _device_batch(self, batch):
-        planes = [torch.as_tensor(b).to(self.device, torch.int32).reshape(-1).contiguous() for b in batch[:3]]
-        ops.check_index_range(torch.stack(planes[:2], 1).contiguous(), (self.item_num, self.item_num),
-                              ('target item', 'context item'))
-        return planes
+    def _launch(self, bu, bi, bj, batch, first, n_steps, apply=True):
+        return ops.i2v_train_steps(self.shared_embedding.weight, self._ws, bu, bi, bj, batch, first, n_steps, self._hp,
+                                   adam_step0=self._opt_steps, apply=apply)
 
     # ------------------------------------------------------------------ reference surface
     def fit(self, train_loader):
@@ -114,19 +71,15 @@ class Item2Vec(GeneralRecommender):
         ops.i2v_user_embedding(self.shared_embedding.weight, self._csr_dev[0], self._csr_dev[1], self.user_embedding.weight)
 
     def calc_loss(self, batch):
-        """Item2VecRecommender.py:63-69: 0-d fp32 loss of one (target, context, label) batch; no update."""
-        self._ensure_ws()
-        bt, bc, bl = self._device_batch(batch)
-        if bt.numel() == 0:
+        """Item2VecRecommender.py:63-69: 0-d fp32 loss of one (target, context, label) batch; no update.  An empty batch
+        launches nothing: its loss is 0."""
+        if len(batch[0]) == 0:
+            self._ensure()
             return torch.zeros((), dtype=torch.float32, device=self.device)
-        loss = ops.i2v_train_steps(self.shared_embedding.weight, self._ws, bt, bc, bl, bt.numel(), 0, 1, self._hp,
-                                   adam_step0=self._opt_steps, apply=False)
-        return loss.to(torch.float32).reshape(())
+        return super().calc_loss(batch)
 
     def train_step(self, batch):
-        """zero_grad + calc_loss + backward + optimizer.step on one batch (AbstractRecommender.py:119-128); -> loss.item()."""
-        self._ensure_ws()
-        bt, bc, bl = self._device_batch(batch)
-        if bt.numel() == 0:
+        if len(batch[0]) == 0:
+            self._ensure()
             return 0.
-        return float(self._train_steps(bt, bc, bl, bt.numel(), 0, 1).item())
+        return super().train_step(batch)

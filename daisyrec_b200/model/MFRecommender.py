@@ -22,22 +22,12 @@ class MF(GeneralRecommender):
     SUPPORTED_LOSSES = ('BPR', 'HL', 'TL', 'CL', 'SL')
     SUPPORTED_OPTIMIZERS = ('sgd', 'adam', 'adagrad', 'rmsprop')     # AbstractRecommender.py:53-60
 
+    MULTI_GPU = None
+
     def __init__(self, config):
         """Same keys as the reference (MFRecommender.py:46-59): lr, reg_1, reg_2, epochs, topk,
         user_num, item_num, factors, loss_type, optimizer, init_method, early_stop (+ gpu, logger)."""
         super().__init__(config)
-        self.lr = config['lr']
-        self.reg_1 = config['reg_1']
-        self.reg_2 = config['reg_2']
-        self.epochs = config['epochs']
-        self.topk = config['topk']
-        self.user_num, self.item_num, self.factors = config['user_num'], config['item_num'], config['factors']
-
-        self.loss_type = config['loss_type']
-        self.optimizer = config['optimizer'] if config['optimizer'] != 'default' else 'sgd'
-        self.initializer = config['init_method'] if config['init_method'] != 'default' else 'normal'
-        self.early_stop = config['early_stop']
-
         # Same CPU RNG consumption as the reference: two nn.Embedding constructors (N(0,1) each),
         # then self.apply(_init_weight) over embed_user, embed_item (AbstractRecommender.py:69-77).
         wu = _init_table(self.user_num, self.factors, None)
@@ -56,8 +46,6 @@ class MF(GeneralRecommender):
             self._P_full_cpu, self.embed_user, self._bounds, self._trainer = wu, None, None, None
         else:
             self.embed_user = _Table(wu.to(self.device))
-        self._ws = None
-        self._opt_steps = 0
         self._stage = None
         self.step_variant = ops.mf_step_variant(self.factors, self.user_num + self.item_num)   # runs the one-off on-device selection
         # optional GPU-path key: True = every cross-thread sum of a step in fixed point (bitwise reproducible runs); single GPU
@@ -81,25 +69,20 @@ class MF(GeneralRecommender):
                              torch.from_numpy(np.ascontiguousarray(col, np.int32)).to(self.device))
             self._neg_seed = int(torch.empty((), dtype=torch.int64).random_().item()) & ((1 << 63) - 1)
 
-    # ------------------------------------------------------------------ plumbing
-    def parameters(self):
-        return [self._full_user_table(), self.embed_item.weight]
-
+    # ------------------------------------------------------------------ plumbing (under torchrun: the full user table)
     def state_dict(self):
+        if self.world == 1:
+            return super().state_dict()
         return {'embed_user.weight': self._full_user_table(), 'embed_item.weight': self.embed_item.weight}
 
     def load_state_dict(self, sd):
-        pu = sd['embed_user.weight']
-        if self.world > 1:                                            # keep this rank's rows of the full table
-            if self._bounds is None:
-                self._shard(self._default_bounds())
-            lo, hi = int(self._bounds[self.rank_id]), int(self._bounds[self.rank_id + 1])
-            pu = pu[lo:hi]
-        self.embed_user.weight.copy_(pu)
+        if self.world == 1:
+            return super().load_state_dict(sd)
+        if self._bounds is None:                                       # keep this rank's rows of the full table
+            self._shard(self._default_bounds())
+        lo, hi = int(self._bounds[self.rank_id]), int(self._bounds[self.rank_id + 1])
+        self.embed_user.weight.copy_(sd['embed_user.weight'][lo:hi])
         self.embed_item.weight.copy_(sd['embed_item.weight'])
-
-    def to(self, device):
-        return self
 
     # ------------------------------------------------------------------ multi-GPU (user-sharded P)
     def _shard(self, bounds):
@@ -141,45 +124,32 @@ class MF(GeneralRecommender):
         pos = torch.arange(lo, hi, device=self.device)
         return allgather_rows(self.embed_user.weight, pos, self.user_num)
 
-    def _hyper(self, opt=None):
-        return ops.hyper(self.lr, self.reg_1, self.reg_2, opt or self._optimizer_name(), loss=str(self.loss_type).upper())
-
     def _begin_fit(self, opt):
         """fit() builds a fresh optimizer (AbstractRecommender.py:105): fresh Adam moments / step count."""
         if str(self.loss_type).upper() in ('CL', 'SL') and (self.world > 1 or self.neg_sampling == 'fused'):
             raise NotImplementedError('the point-wise losses (CL / SL) run on one GPU with sampler-made rows; the sharded '
                                       'step and the fused negative sampler cover the pair-wise losses')
+        if self.world == 1:
+            return super()._begin_fit(opt)
         self._hp = self._hyper(opt)
         self._opt_steps = 0
-        if self.world > 1:
-            if self._trainer is not None:
-                self._trainer.close()                              # keeps a private copy of Q; frees the peer buffers
-                self.embed_item = _Table(self._trainer.Q)
-            self._trainer = None                                   # fresh optimiser state per fit()
-            return
-        self._ws = ops.MFWorkspace(self.user_num, self.item_num, self.factors, opt, self.device, deterministic=self.deterministic)
+        if self._trainer is not None:
+            self._trainer.close()                                  # keeps a private copy of Q; frees the peer buffers
+            self.embed_item = _Table(self._trainer.Q)
+        self._trainer = None                                       # fresh optimiser state per fit()
 
-    def _ensure_ws(self):
-        if self._ws is None:
-            self._begin_fit(self._optimizer_name())
+    def _workspace(self, opt, rows=None):
+        return ops.MFWorkspace(self.user_num, self.item_num, self.factors, opt, self.device, deterministic=self.deterministic)
 
-    def _train_steps(self, bu, bi, bj, batch, first, n_steps):
+    def _launch(self, bu, bi, bj, batch, first, n_steps, apply=True):
+        P, Q = self.embed_user.weight, self.embed_item.weight
+        if not apply:
+            return ops.mf_bpr_loss(P, Q, self._ws, bu, bi, bj, self._hp)
         if self.neg_sampling == 'fused':
-            losses = ops.mf_bpr_train_steps_fused_neg(self.embed_user.weight, self.embed_item.weight, self._ws, bu, bi,
-                                                      self._csr_dev[0], self._csr_dev[1], self._neg_seed + self._opt_steps,
-                                                      batch, first, n_steps, self._hp, adam_step0=self._opt_steps)
-            self._opt_steps += n_steps
-            return losses
-        losses = ops.mf_bpr_train_steps(self.embed_user.weight, self.embed_item.weight, self._ws, bu, bi, bj, batch,
-                                        first, n_steps, self._hp, adam_step0=self._opt_steps)
-        self._opt_steps += n_steps
-        return losses
-
-    @staticmethod
-    def _host_i32(x):
-        if isinstance(x, torch.Tensor):
-            x = x.detach().cpu().numpy()
-        return np.ascontiguousarray(x, dtype=np.int32)
+            return ops.mf_bpr_train_steps_fused_neg(P, Q, self._ws, bu, bi, self._csr_dev[0], self._csr_dev[1],
+                                                    self._neg_seed + self._opt_steps, batch, first, n_steps, self._hp,
+                                                    adam_step0=self._opt_steps)
+        return ops.mf_bpr_train_steps(P, Q, self._ws, bu, bi, bj, batch, first, n_steps, self._hp, adam_step0=self._opt_steps)
 
     # ------------------------------------------------------------------ reference surface
     def _full_user_table(self):
@@ -191,13 +161,14 @@ class MF(GeneralRecommender):
             self._shard(self._default_bounds())
         return self.gather_user_table()
 
-    def forward(self, user, item):
-        """MFRecommender.py:63-68: pred = (P[user] * Q[item]).sum(-1) for index tensors."""
-        u = torch.as_tensor(user).to(self.device, torch.int32).reshape(-1).contiguous()
-        i = torch.as_tensor(item).to(self.device, torch.int32).reshape(-1).contiguous()
-        return ops.mf_predict(self._full_user_table(), self.embed_item.weight, u, i)
+    def _dot_tables(self):
+        return self._full_user_table(), self.embed_item.weight
 
-    __call__ = forward
+    @staticmethod
+    def _host_i32(x):
+        if isinstance(x, torch.Tensor):
+            x = x.detach().cpu().numpy()
+        return np.ascontiguousarray(x, dtype=np.int32)
 
     def calc_loss(self, batch):
         """MFRecommender.py:70-97: 0-d fp32 loss of one (user, pos, neg) -- or, for CL / SL, (user, item, label) --
@@ -206,10 +177,7 @@ class MF(GeneralRecommender):
         if self.world > 1:
             raise NotImplementedError('calc_loss / train_step on single batches are single-GPU entry points; under torchrun '
                                       'use fit(train_loader) (user-sharded global steps)')
-        self._ensure_ws()
-        bu, bi, bj = (torch.as_tensor(b).to(self.device, torch.int32).contiguous() for b in batch[:3])
-        loss = ops.mf_bpr_loss(self.embed_user.weight, self.embed_item.weight, self._ws, bu, bi, bj, self._hp)
-        return loss.to(torch.float32).reshape(())
+        return super().calc_loss(batch)
 
     def train_step(self, batch):
         """zero_grad + calc_loss + backward + optimizer.step on one HOST batch
@@ -217,7 +185,8 @@ class MF(GeneralRecommender):
         self._check_loss_type()
         if self.world > 1:
             raise NotImplementedError('train_step is a single-GPU entry point; under torchrun use fit(train_loader)')
-        self._ensure_ws()
+        self._check_ids(batch[:3], *self._index_bounds())
+        self._ensure()
         hb = [self._host_i32(b) for b in batch[:3]]
         n = len(hb[0])
         if self._stage is None or self._stage.numel() < 3 * ((n + 3) // 4 * 4) + 4:
@@ -233,7 +202,7 @@ class MF(GeneralRecommender):
         ``.to(device)`` copies and ``loss.item()`` reads kept, but pipelined (copy of batch s+1 under the
         kernel of batch s).  Returns the per-step losses (CPU float64 tensor)."""
         self._check_loss_type()
-        self._ensure_ws()
+        self._ensure()
         n = h_bu.numel()
         if n_steps is None:
             n_steps = (n + batch_size - 1) // batch_size
@@ -242,36 +211,12 @@ class MF(GeneralRecommender):
         self._opt_steps += n_steps
         return losses
 
-    def predict(self, u, i):
-        """MFRecommender.py:99-104 -> python float."""
-        return float(self.forward([u], [i]).item())
-
     def rank(self, test_loader):
         """MFRecommender.py:106-123 -> float32 ndarray [n_test_users, topk], rows in loader order."""
-        ds = getattr(test_loader, 'dataset', None)
-        data = getattr(ds, 'data', None)
-        if isinstance(data, (list, tuple)) and len(data) and len(data[0]) == 2:
-            users = np.fromiter((int(r[0]) for r in data), np.int64, len(data))
-            cands = np.stack([np.asarray(r[1], dtype=np.int64) for r in data])
-        else:                                                   # any iterable of (us, cands_ids) batches
-            us, cs = [], []
-            for b_us, b_c in test_loader:
-                us.append(torch.as_tensor(b_us).reshape(-1).to(torch.int64))
-                cs.append(torch.as_tensor(b_c).to(torch.int64).reshape(us[-1].numel(), -1))
-            if not us:
-                return np.zeros((0,), np.float32)
-            users, cands = torch.cat(us).numpy(), torch.cat(cs).numpy()
-        if len(users) == 0:
-            return np.zeros((0,), np.float32)
-        k = min(self.topk, cands.shape[1])
-        if users.min() < 0 or users.max() >= self.user_num:
-            raise IndexError('index out of range in self: test user id outside [0, user_num)')
-        if self.world > 1:
-            return self._rank_sharded(users, cands, k)
-        d_cands = torch.from_numpy(np.ascontiguousarray(cands)).to(self.device)
-        ops.check_index_range(d_cands.reshape(-1, 1), (self.item_num,), ('candidate item',))
-        out = ops.mf_rank(self.embed_user.weight, self.embed_item.weight, torch.from_numpy(users).to(self.device), d_cands, k)
-        return out.cpu().numpy()
+        if self.world == 1:
+            return super().rank(test_loader)
+        ins = self._rank_inputs(test_loader)
+        return np.zeros((0,), np.float32) if ins is None else self._rank_sharded(*ins)
 
     def _rank_sharded(self, users, cands, k):
         """Each rank scores the test users it owns; one all-gather assembles [n_users, k] in loader order."""
@@ -289,14 +234,8 @@ class MF(GeneralRecommender):
         out = allgather_rows(loc, torch.from_numpy(mine).to(self.device), len(users))
         return out.cpu().numpy()
 
-    def full_rank(self, u):
-        """MFRecommender.py:126-133 -> int64 ndarray [topk]; no masking of train items."""
-        users = torch.tensor([int(u)], dtype=torch.int64, device=self.device)
-        k = min(self.topk, self.item_num)
-        return ops.mf_full_rank(self._full_user_table(), self.embed_item.weight, users, k)[0].cpu().numpy()
-
     def full_rank_users(self, users):
         """Batched full_rank (GPU extension): int64 ndarray [len(users), topk]."""
-        users = torch.as_tensor(np.asarray(users, dtype=np.int64)).to(self.device)
+        users = self._device_ids((np.asarray(users, dtype=np.int64),), (self.user_num,), ('user',), torch.int64)[0]
         k = min(self.topk, self.item_num)
         return ops.mf_full_rank(self._full_user_table(), self.embed_item.weight, users, k).cpu().numpy()

@@ -11,27 +11,19 @@ import numpy as np
 import torch
 
 from .. import ops
-from .AbstractRecommender import GeneralRecommender, _Table, _INIT
+from .AbstractRecommender import GeneralRecommender, _Table, _INIT, ragged_split
 
 
 class NeuMF(GeneralRecommender):
+    DEFAULT_OPTIMIZER, DEFAULT_INIT = 'adam', 'xavier_normal'
+    PARAMS = ('embed_user_GMF.weight', 'embed_item_GMF.weight', 'embed_user_MLP.weight', 'embed_item_MLP.weight', 'tower')
+    SCRATCH_KEY = 'neumf_scratch_rows'
+
     def __init__(self, config):
         super().__init__(config)
-        if self.world > 1:
-            raise NotImplementedError('NeuMF runs as independent replicas only (DESIGN.md, multi-GPU section)')
-        self.lr = config['lr']
-        self.epochs = config['epochs']
-        self.reg_1 = config['reg_1']
-        self.reg_2 = config['reg_2']
         self.dropout = config['dropout']
         self.model = config['model_name']
-        self.user_num, self.item_num = config['user_num'], config['item_num']
-        self.factors, self.num_layers = config['factors'], config['num_layers']
-        self.loss_type = config['loss_type']
-        self.optimizer = config['optimizer'] if config['optimizer'] != 'default' else 'adam'
-        self.initializer = config['init_method'] if config['init_method'] != 'default' else 'xavier_normal'
-        self.early_stop = config['early_stop']
-        self.topk = config['topk']
+        self.num_layers = config['num_layers']
         if self.model not in ops.NEUMF_MODE:
             raise ValueError(f"model_name={self.model!r}: expected one of {sorted(ops.NEUMF_MODE)}")
         self._mode = ops.NEUMF_MODE[self.model]                       # 0 NeuMF / NeuMF-pre, 1 GMF, 2 MLP
@@ -77,9 +69,6 @@ class NeuMF(GeneralRecommender):
         self.embed_user_MLP = _Table(embs[2].weight.detach().to(self.device).contiguous())
         self.embed_item_MLP = _Table(embs[3].weight.detach().to(self.device).contiguous())
         self.tower = tower.to(self.device)
-        self._ws = None
-        self._opt_steps = 0
-        self._rows = int(config.get('neumf_scratch_rows', 1 << 16))
         # optional GPU-path key: 'fp32' (CUDA cores, parity path, default) | 'bf16' (wgmma tensor cores, BASELINE config 3)
         #                   | 'fused' (bf16 wgmma, the whole tower step of a 64-triple tile inside one CTA: activations stay in
         #                     shared memory, accumulators in registers; factors = 32, num_layers = 2, dropout 0 -- other shapes run as 'bf16')
@@ -139,40 +128,12 @@ class NeuMF(GeneralRecommender):
         return (self.embed_user_GMF.weight, self.embed_item_GMF.weight, self.embed_user_MLP.weight,
                 self.embed_item_MLP.weight)
 
-    def parameters(self):
-        return list(self._tabs()) + [self.tower]
-
-    def state_dict(self):
-        return {'embed_user_GMF.weight': self.embed_user_GMF.weight, 'embed_item_GMF.weight': self.embed_item_GMF.weight,
-                'embed_user_MLP.weight': self.embed_user_MLP.weight, 'embed_item_MLP.weight': self.embed_item_MLP.weight,
-                'tower': self.tower}
-
-    def load_state_dict(self, sd):
-        for k, t in self.state_dict().items():
-            t.copy_(torch.as_tensor(sd[k]).reshape(t.shape))
-
-    def _hyper(self, opt=None):
-        return ops.hyper(self.lr, self.reg_1, self.reg_2, opt or self._optimizer_name())
-
-    def _workspace(self, rows, opt=None, fresh=False):
-        rows = max(int(rows), self._rows)
-        if fresh or self._ws is None or self._ws.max_rows < rows:
-            keep = None if fresh or self._ws is None else self._ws
-            if keep is not None and opt is None:
-                # growing the scratch would drop the optimiser state: size it up front instead
-                raise RuntimeError('NeuMF scratch too small; set config["neumf_scratch_rows"] >= 2 * batch_size')
-            self._ws = ops.NeumfWorkspace(self.user_num, self.item_num, self.factors, self.num_layers,
-                                          opt or self._optimizer_name(), rows, self.device)
-        return self._ws
+    def _workspace(self, opt, rows):
+        return ops.NeumfWorkspace(self.user_num, self.item_num, self.factors, self.num_layers, opt, rows, self.device)
 
     def _begin_fit(self, opt):
-        # dropout masks are counter-based (Philox) on the device; the key is drawn from torch's global RNG so that
-        # torch.manual_seed makes runs reproducible (the masks themselves are NOT torch's: parity holds at dropout=0)
         self._philox_seed = None                                     # drawn lazily: the host-mask engine must not move the RNG here
-        self._hp = self._hyper(opt)
-        self._opt_steps = 0
-        self._fit_opt = opt
-        self._ws = None                                              # fresh optimiser state per fit()
+        super()._begin_fit(opt)
 
     def _host_masks(self, rows_per_step):
         """Parity dropout: the keep-masks nn.Dropout would draw for steps of rows_per_step[k] triples, drawn by torch on the CPU
@@ -207,96 +168,42 @@ class NeuMF(GeneralRecommender):
             return 2 * batch * (4 * self.mlp_dim - 2 * self.factors) <= (1 << 22)
         return self.dropout_engine == 'torch'
 
-    def _train_steps(self, bu, bi, bj, batch, first, n_steps):
-        if self._ws is None:
-            self._workspace(2 * batch, self._fit_opt, fresh=True)
-        p = self.dropout if self.training else 0.0
-        kw = dict(tower_dtype=self._tower_dtype, dropout=p, mode=self._mode)
-        n = bu.numel()
-        if self._use_host_masks(batch):
-            full = n_steps if (first + n_steps) * batch <= n else n_steps - 1   # a ragged last batch gets its own masks + call
-            out = []
-            if full > 0:
-                masks = self._host_masks([batch] * full)
-                out.append(ops.neumf_bpr_train_steps(self._tabs(), self.tower, self._ws, bu, bi, bj, batch, first, full, self._hp,
-                                                     adam_step0=self._opt_steps, drop_masks=masks, **kw))
-            if full < n_steps:
-                base = (first + full) * batch
-                last = n - base
-                masks = self._host_masks([last])
-                out.append(ops.neumf_bpr_train_steps(self._tabs(), self.tower, self._ws, bu[base:], bi[base:], bj[base:], last, 0,
-                                                     1, self._hp, adam_step0=self._opt_steps + full, drop_masks=masks, **kw))
-            losses = torch.cat(out)
-        else:
-            losses = ops.neumf_bpr_train_steps(self._tabs(), self.tower, self._ws, bu, bi, bj, batch, first, n_steps, self._hp,
-                                               adam_step0=self._opt_steps, dropout_seed=self._drop_seed(), **kw)
-        self._opt_steps += n_steps
-        return losses
-
-    def _ensure(self, rows):
-        if self._ws is None:
-            self._begin_fit(self._optimizer_name())
-            self._workspace(rows, self._fit_opt, fresh=True)
-        elif self._ws.max_rows < rows:
-            self._workspace(rows)
+    def _launch(self, bu, bi, bj, batch, first, n_steps, apply=True):
+        kw = dict(apply=apply, tower_dtype=self._tower_dtype, dropout=self.dropout if self.training else 0.0, mode=self._mode)
+        if not self._use_host_masks(batch):
+            return ops.neumf_bpr_train_steps(self._tabs(), self.tower, self._ws, bu, bi, bj, batch, first, n_steps, self._hp,
+                                             adam_step0=self._opt_steps, dropout_seed=self._drop_seed(), **kw)
+        full, last = ragged_split(bu.numel(), batch, first, n_steps)
+        out = []
+        if full > 0:
+            out.append(ops.neumf_bpr_train_steps(self._tabs(), self.tower, self._ws, bu, bi, bj, batch, first, full, self._hp,
+                                                 adam_step0=self._opt_steps, drop_masks=self._host_masks([batch] * full), **kw))
+        if last:
+            base = (first + full) * batch
+            out.append(ops.neumf_bpr_train_steps(self._tabs(), self.tower, self._ws, bu[base:], bi[base:], bj[base:], last, 0, 1,
+                                                 self._hp, adam_step0=self._opt_steps + full, drop_masks=self._host_masks([last]),
+                                                 **kw))
+        return torch.cat(out)
 
     # ------------------------------------------------------------------ reference surface
-    def forward(self, user, item):
-        u = torch.as_tensor(user).to(self.device, torch.int64).reshape(-1).contiguous()
-        i = torch.as_tensor(item).to(self.device, torch.int64).reshape(-1, 1).contiguous()
+    def _scores(self, users, items, per_user):
         self._ensure(1)
-        return ops.neumf_scores(self._tabs(), self.tower, self._ws, u, i, 1, self._tower_dtype, self._mode).reshape(-1)
+        return ops.neumf_scores(self._tabs(), self.tower, self._ws, users, items, per_user, self._tower_dtype, self._mode)
 
-    __call__ = forward
-
-    def calc_loss(self, batch):
-        self._check_loss_type()
-        bu, bi, bj = (torch.as_tensor(b).to(self.device, torch.int32).contiguous() for b in batch[:3])
-        self._ensure(2 * bu.numel())
-        masks = self._host_masks([bu.numel()]) if self._use_host_masks(bu.numel()) else None
-        loss = ops.neumf_bpr_train_steps(self._tabs(), self.tower, self._ws, bu, bi, bj, bu.numel(), 0, 1, self._hp,
-                                         apply=False, tower_dtype=self._tower_dtype, adam_step0=self._opt_steps,
-                                         dropout=self.dropout if self.training else 0.0,
-                                         dropout_seed=0 if masks is not None else self._drop_seed(), drop_masks=masks,
-                                         mode=self._mode)
-        return loss.to(torch.float32).reshape(())
-
-    def train_step(self, batch):
-        self._check_loss_type()
-        bu, bi, bj = (torch.as_tensor(b).to(self.device, torch.int32).contiguous() for b in batch[:3])
-        self._ensure(2 * bu.numel())
-        was = self.training
-        self.train()                                                 # a training step runs in train mode (dropout on)
-        try:
-            return float(self._train_steps(bu, bi, bj, bu.numel(), 0, 1).item())
-        finally:
-            self.train(was)
-
-    def predict(self, u, i):
-        return float(self.forward([int(u)], [int(i)]).item())
+    def _pair_scores(self, user, item):
+        u, i = self._pair_ids(user, item, torch.int64)
+        return self._scores(u, i.reshape(-1, 1), 1).reshape(-1)
 
     def rank(self, test_loader):
-        data = getattr(getattr(test_loader, 'dataset', None), 'data', None)
-        if isinstance(data, (list, tuple)) and len(data) and len(data[0]) == 2:
-            users = np.fromiter((int(r[0]) for r in data), np.int64, len(data))
-            cands = np.stack([np.asarray(r[1], dtype=np.int64) for r in data])
-        else:
-            us, cs = [], []
-            for b_us, b_c in test_loader:
-                us.append(torch.as_tensor(b_us).reshape(-1).to(torch.int64))
-                cs.append(torch.as_tensor(b_c).to(torch.int64).reshape(us[-1].numel(), -1))
-            if not us:
-                return np.zeros((0,), np.float32)
-            users, cands = torch.cat(us).numpy(), torch.cat(cs).numpy()
-        self._ensure(1)
-        d_users = torch.from_numpy(users).to(self.device)
-        d_cands = torch.from_numpy(np.ascontiguousarray(cands)).to(self.device)
-        scores = ops.neumf_scores(self._tabs(), self.tower, self._ws, d_users, d_cands, cands.shape[1], self._tower_dtype, self._mode)
-        k = min(self.topk, cands.shape[1])
+        ins = self._rank_inputs(test_loader)
+        if ins is None:
+            return np.zeros((0,), np.float32)
+        users, cands, k = ins
+        d_cands = torch.from_numpy(cands).to(self.device)
+        scores = self._scores(torch.from_numpy(users).to(self.device), d_cands, cands.shape[1])
         return ops.topk_from_scores(scores, d_cands, k).cpu().numpy()
 
     def full_rank(self, u):
-        self._ensure(1)
-        users = torch.tensor([int(u)], dtype=torch.int64, device=self.device)
-        scores = ops.neumf_scores(self._tabs(), self.tower, self._ws, users, None, self.item_num, self._tower_dtype, self._mode)
+        users = self._device_ids(([int(u)],), (self.user_num,), ('user',), torch.int64)[0]
+        scores = self._scores(users, None, self.item_num)
         return ops.topk_from_scores(scores, None, min(self.topk, self.item_num))[0].cpu().numpy()
