@@ -163,9 +163,9 @@ static int ub_users_for(int U, int F, long long batch)
     return (nbk <= kUbMaxBuckets && batch + 4 * nbk < (1LL << 31)) ? ub : 0;
 }
 
-// The bucketed mode's scratch (counters, bucket ranges, partitioned planes): library-owned, grow-only, one per device and stream;
+// The bucketed mode's scratch (counters, bucket ranges, partitioned triples): library-owned, grow-only, one per device and stream;
 // it depends on the batch, so it cannot live in the workspace.  Its counters are cleared before every launch.  Each buffer lives
-// as long as the process: about 12 B x the largest batch of bucketed steps launched on that stream (12.6 MB at B = 1 M), so a
+// as long as the process: about 16 B x the largest batch of bucketed steps launched on that stream (16.8 MB at B = 1 M), so a
 // caller that trains on many streams holds one such buffer per stream.
 static int ub_scratch(StepParams &p, cudaStream_t st)
 {
@@ -173,8 +173,7 @@ static int ub_scratch(StepParams &p, cudaStream_t st)
     static std::map<std::pair<int, cudaStream_t>, std::pair<void *, size_t>> bufs;
     const size_t nbk = (size_t)p.ub_buckets;
     const size_t cnt_b = align256(sizeof(unsigned) * (2 * nbk + 1)), rng_b = align256(sizeof(int) * 2 * nbk);
-    const size_t plane = align256(sizeof(int32_t) * ((size_t)p.batch + 4 * nbk));
-    const size_t need = cnt_b + rng_b + 3 * plane;
+    const size_t need = cnt_b + rng_b + sizeof(int4) * (size_t)p.batch;
     int dev = 0;
     DRB_CUDA(cudaGetDevice(&dev));
     std::lock_guard<std::mutex> lock(mu);
@@ -191,9 +190,7 @@ static int ub_scratch(StepParams &p, cudaStream_t st)
     char *b = (char *)e.first;
     p.ub_count = (unsigned *)b;
     p.ub_range = (int *)(b + cnt_b);
-    p.ub_u = (int32_t *)(b + cnt_b + rng_b);
-    p.ub_i = (int32_t *)(b + cnt_b + rng_b + plane);
-    p.ub_j = (int32_t *)(b + cnt_b + rng_b + 2 * plane);
+    p.ub_t = (int4 *)(b + cnt_b + rng_b);
     DRB_CUDA(cudaMemsetAsync(p.ub_count, 0, sizeof(unsigned) * (2 * nbk + 1), st));
     return DRB_OK;
 }

@@ -114,8 +114,9 @@ struct StepParams {
     // owned by the launcher (mf_bpr.cu), not part of the workspace: its size depends on the batch.
     int ub_users = 0, ub_buckets = 0;
     unsigned *ub_count = nullptr;  // [2 * ub_buckets + 1]: triples per bucket, reservation cursors, work counter; zero between steps
-    int *ub_range = nullptr;       // [2 * ub_buckets]: first and end position of bucket b in the partitioned planes
-    int32_t *ub_u = nullptr, *ub_i = nullptr, *ub_j = nullptr;  // partitioned planes; every bucket starts at a multiple of 4
+    int *ub_range = nullptr;       // [2 * ub_buckets]: first and end position of bucket b in the partitioned triples
+    int4 *ub_t = nullptr;          // [batch]: the partitioned triples as (u, i, j, 0) records, bucket after bucket
+    void *ub_spare[2] = {};        // unused: keeps the size, so the parameters after StepParams (p2p.cu) keep their offsets
 };
 
 // One step on a batch of B triples (bu, bi, bj) of a U x I problem with F factors, with the hyper-parameters of h; the

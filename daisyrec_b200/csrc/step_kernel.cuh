@@ -265,8 +265,8 @@ struct NoExchange {
 // no in-kernel negative draw, and 32-bit element offsets into the tables (rows * F < 2^32) -- the same arithmetic on the same
 // operands in the same order as the general body, with ~1/3 fewer instructions per triple.
 //
-// UBK (user-bucketed, lean single-GPU fused steps only): every step first partitions its triples by user bucket into scratch planes
-// (histogram, grid barrier, scan + reservation, scatter, grid barrier); phase 1 then has CTAs claim whole buckets, sum the user
+// UBK (user-bucketed, lean single-GPU fused steps only): every step first partitions its triples by user bucket into scratch
+// records (histogram, grid barrier, scan + reservation, scatter, grid barrier); phase 1 then has CTAs claim whole buckets, sum the user
 // gradient rows and counts of the bucket in shared memory and write each touched gP row and cntU entry once with plain stores,
 // instead of one RED per occurrence into the (L2-missing) user accumulators.  Item side, loss and norms are unchanged; only the
 // fp32 summation order of the user gradient differs (the REDs leave it unspecified as well).
@@ -280,7 +280,8 @@ __device__ __forceinline__ void bpr_steps_body(StepParams &p, XCH &xch)
     constexpr int GROUPS = (kThreads / 32) * GPW;  // lane groups per CTA
     constexpr int UNR = (NCH * VEC <= (LEAN ? 8 : 4)) ? DRB_UNR : 1;  // triples in flight per group
 
-    __shared__ __align__(128) int32_t s_idx[2][3][kTileMax];
+    // index tiles: three planes u, i, j; UBK: kTileMax (u, i, j, 0) records
+    __shared__ __align__(128) int32_t s_idx[2][UBK ? 4 : 3][kTileMax];
     __shared__ uint64_t s_bar[2];
     __shared__ double s_red[8][kThreads / 32];
     extern __shared__ __align__(16) unsigned char s_dyn[];   // UBK: partition histogram, then the bucket accumulator
@@ -328,14 +329,12 @@ __device__ __forceinline__ void bpr_steps_body(StepParams &p, XCH &xch)
             if (tid == 0) mbar_arrive(&s_bar[b]);
         }
     };
-    // UBK, thread 0: bulk copy of the partitioned triples [t0, t0 + cnt) into tile buffer b (every bucket starts at a multiple
-    // of 4 triples and has room for the rounding up)
+    // UBK, thread 0: one bulk copy of the partitioned triples [t0, t0 + cnt) into tile buffer b (16-byte records: every start
+    // and size is a multiple of 16 bytes)
     auto stage_ub = [&](int t0, int cnt, int b) {
-        const uint32_t bytes = (uint32_t)((cnt + 3) & ~3) * 4u;
-        mbar_expect_tx(&s_bar[b], 3u * bytes);
-        tma_load_1d(&s_idx[b][0][0], p.ub_u + t0, bytes, &s_bar[b]);
-        tma_load_1d(&s_idx[b][1][0], p.ub_i + t0, bytes, &s_bar[b]);
-        tma_load_1d(&s_idx[b][2][0], p.ub_j + t0, bytes, &s_bar[b]);
+        const uint32_t bytes = (uint32_t)cnt * 16u;
+        mbar_expect_tx(&s_bar[b], bytes);
+        tma_load_1d(&s_idx[b][0][0], p.ub_t + t0, bytes, &s_bar[b]);
     };
     // UBK, thread 0: claim the next non-empty bucket through the work counter, publish it in s_claim and stage its first tile
     auto claim = [&](int b) {
@@ -366,7 +365,7 @@ __device__ __forceinline__ void bpr_steps_body(StepParams &p, XCH &xch)
         __syncthreads();
         int buf = 0;
         long long t_i = blockIdx.x;
-        // UBK: claimed bucket bk, its triples [r0, r1) in the partitioned planes, position tt of the current tile; the gradient
+        // UBK: claimed bucket bk, its triples [r0, r1) in the partitioned records, position tt of the current tile; the gradient
         // rows and counts of its users u0 .. u0 + rows - 1 sum in s_gp / s_cu (row stride F + 1 against bank conflicts between
         // the groups of a warp)
         int bk = 0, r0 = 0, r1 = 0, tt = 0, u0 = 0, rows = 0;
@@ -385,11 +384,11 @@ __device__ __forceinline__ void bpr_steps_body(StepParams &p, XCH &xch)
             for (int b = tid; b < NBK; b += kThreads)
                 if (s_hist[b] != 0u) red_add_u32(ucnt + b, s_hist[b]);
             grid_barrier(&hdr->barrier, epoch);
-            // exclusive scan of the counts, each padded to a multiple of 4 (bulk copies of a bucket start 16-byte aligned), in
-            // every CTA; CTA 0 publishes the ranges; each CTA reserves its slice of every bucket it holds triples of
+            // exclusive scan of the counts in every CTA; CTA 0 publishes the ranges; each CTA reserves its slice of every bucket
+            // it holds triples of
             const int per = (NBK + kThreads - 1) / kThreads, b0 = min(NBK, tid * per), b1 = min(NBK, b0 + per);
             unsigned run = 0u;
-            for (int b = b0; b < b1; ++b) run += (__ldcg(ucnt + b) + 3u) & ~3u;
+            for (int b = b0; b < b1; ++b) run += __ldcg(ucnt + b);
             unsigned incl = run;
 #pragma unroll
             for (int off = 1; off < 32; off <<= 1) {
@@ -405,18 +404,18 @@ __device__ __forceinline__ void bpr_steps_body(StepParams &p, XCH &xch)
                 if (blockIdx.x == 0) { p.ub_range[2 * b] = (int)start; p.ub_range[2 * b + 1] = (int)(start + c); }
                 s_off[b] = h != 0u ? start + atomicAdd(ucur + b, h) : 0u;
                 s_hist[b] = 0u;
-                start += (c + 3u) & ~3u;
+                start += c;
             }
             __syncthreads();
-            // ---- scatter this CTA's triples into the partitioned planes (the same triples as the histogram pass)
+            // ---- scatter this CTA's triples into the partitioned records (the same triples as the histogram pass); a CTA holds
+            // about two triples per bucket, so these stores land at random: one 16-byte store per triple, not three 4-byte ones
             for (long long t = g0; t < nb; t += gstride) {
                 const int u = __ldg(p.bu + base + t), b = u / UBU;
+                const int i = __ldg(p.bi + base + t), j = __ldg(p.bj + base + t);
                 const unsigned pos = s_off[b] + atomicAdd(&s_hist[b], 1u);
-                p.ub_u[pos] = u;
-                p.ub_i[pos] = __ldg(p.bi + base + t);
-                p.ub_j[pos] = __ldg(p.bj + base + t);
+                p.ub_t[pos] = make_int4(u, i, j, 0);
             }
-            asm volatile("fence.proxy.async.global;" ::: "memory");   // the planes are read back by bulk copies (async proxy)
+            asm volatile("fence.proxy.async.global;" ::: "memory");   // the records are read back by bulk copies (async proxy)
             grid_barrier(&hdr->barrier, epoch);
             for (long long k = g0; k < 2LL * NBK; k += gstride) ucnt[k] = 0u;   // counts, cursors: zero for the next step
             s_gp = reinterpret_cast<float *>(s_dyn);
@@ -447,7 +446,9 @@ __device__ __forceinline__ void bpr_steps_body(StepParams &p, XCH &xch)
             }
             if (buf == 0) { mbar_wait(&s_bar[0], par0); par0 ^= 1; } else { mbar_wait(&s_bar[1], par1); par1 ^= 1; }
             const int cnt = UBK ? min(r1 - tt, kTileMax) : (int)min((long long)tile, nb - t_i * tile);
-            const int32_t *xu = s_idx[buf][0], *xi = s_idx[buf][1], *xj = s_idx[buf][2];
+            // triple t's indices: xu[XS * t], xi[XS * t], xj[XS * t] (UBK: fields of record t)
+            constexpr int XS = UBK ? 4 : 1;
+            const int32_t *xu = s_idx[buf][0], *xi = UBK ? xu + 1 : s_idx[buf][1], *xj = UBK ? xu + 2 : s_idx[buf][2];
             float t_loss = 0.f, t_l1u = 0.f, t_l1i = 0.f, t_l1j = 0.f, t_s2u = 0.f, t_s2i = 0.f, t_s2j = 0.f, t_gb0 = 0.f;
 
             for (int tb = 0; tb < cnt; tb += GROUPS * UNR) {
@@ -460,9 +461,9 @@ __device__ __forceinline__ void bpr_steps_body(StepParams &p, XCH &xch)
                 for (int r = 0; r < UNR; ++r) {
                     int t = tb + r * GROUPS + group;
                     ok[r] = t < cnt;
-                    iu[r] = ok[r] ? xu[t] : 0;
-                    ii[r] = ok[r] ? xi[t] : 0;
-                    ij[r] = ok[r] ? xj[t] : 0;
+                    iu[r] = ok[r] ? xu[XS * t] : 0;
+                    ii[r] = ok[r] ? xi[XS * t] : 0;
+                    ij[r] = ok[r] ? xj[XS * t] : 0;
                     lab[r] = 0.f;
                     if (pw) {                       // label = batch[2].float() (MFRecommender.py:76); the j row stays zero
                         lab[r] = (float)ij[r];
