@@ -17,7 +17,7 @@ c_f32p = C.POINTER(C.c_float)
 c_f64p = C.POINTER(C.c_double)
 vp = C.c_void_p
 
-DRB_OK, DRB_ERR_INVALID, DRB_ERR_CUDA, DRB_ERR_NAN_LOSS, DRB_ERR_EMPTY_SET, DRB_ERR_NO_DEVICE, DRB_ERR_PEER = range(7)
+DRB_OK, DRB_ERR_INVALID, DRB_ERR_CUDA, DRB_ERR_NAN_LOSS, DRB_ERR_EMPTY_SET, DRB_ERR_NO_DEVICE, DRB_ERR_PEER, DRB_ERR_NOT_PD = range(8)
 OPT_SGD, OPT_ADAM, OPT_ADAGRAD, OPT_RMSPROP = 0, 1, 2, 3
 OPT_KIND = {"sgd": 0, "adam": 1, "adagrad": 2, "rmsprop": 3}
 LOSS_KIND = {"BPR": 0, "HL": 1, "TL": 2, "CL": 3, "SL": 4}
@@ -164,6 +164,15 @@ SIGNATURES = {
     "drb_csr_workspace_bytes": (C.c_size_t, [C.c_int32, C.c_int64]),
     "drb_csr_build": (C.c_int, [vp, vp, C.c_int64, C.c_int32, C.c_int32, vp, vp, vp, c_i64p, vp]),
     "drb_lgcn_build_adj": (C.c_int, [vp, vp, vp, vp, C.c_int32, C.c_int32, C.c_int64, vp, vp, vp, vp]),
+    "drb_ease_csr_workspace_bytes": (C.c_size_t, [C.c_int32, C.c_int64]),
+    "drb_ease_csr": (C.c_int, [vp, vp, vp, vp, C.c_int32, C.c_int32, vp, vp, C.c_int64, vp, vp, c_i32p, vp]),
+    "drb_ease_workspace_bytes": (C.c_size_t, [C.c_int32, C.c_int32, C.c_int32]),
+    "drb_ease_gram": (C.c_int, [vp, vp, vp, C.c_int32, C.c_int32, C.c_int32, C.c_double, vp, vp, vp]),
+    "drb_ease_inverse": (C.c_int, [vp, C.c_int32, vp, vp]),
+    "drb_ease_weights": (C.c_int, [vp, C.c_int32, vp, vp]),
+    "drb_ease_rank": (C.c_int, [vp, C.c_int32, vp, vp, vp, vp, C.c_int64, vp, C.c_int32, C.c_int32, vp, vp, vp]),
+    "drb_ease_full_rank": (C.c_int, [vp, C.c_int32, vp, vp, vp, vp, C.c_int32, C.c_int32, vp, vp, vp]),
+    "drb_ease_predict": (C.c_int, [vp, C.c_int32, vp, vp, vp, vp, vp, C.c_int64, vp, vp]),
     "drb_rank_metrics_workspace_bytes": (C.c_size_t, [C.c_int32, C.c_int32]),
     "drb_rank_metrics": (C.c_int, [vp, C.c_int64, C.c_int32, vp, vp, vp, C.c_int32, C.c_int32, vp, vp, vp, vp]),
     "drb_rank_metrics_host": (C.c_int, [vp, C.c_int64, C.c_int32, vp, vp, vp, C.c_int32, C.c_int32, vp, vp]),
@@ -267,4 +276,7 @@ def check(rc):
         raise ValueError(NAN_LOSS_MESSAGE)
     if rc == DRB_ERR_EMPTY_SET:
         raise ValueError(EMPTY_SET_MESSAGE)
+    if rc == DRB_ERR_NOT_PD:
+        import numpy as np
+        raise np.linalg.LinAlgError((lib().drb_last_error() or b"").decode(errors="replace"))
     raise DrbError(rc, (lib().drb_last_error() or b"").decode(errors="replace"))

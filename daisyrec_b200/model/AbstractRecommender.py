@@ -181,17 +181,10 @@ def ragged_split(n, batch, first, n_steps):
     return full, (n - (first + full) * batch if full < n_steps else 0)
 
 
-class GeneralRecommender(AbstractRecommender):
-    """Shared plumbing of the GPU-path models.  A subclass declares its defaults and state as class data, builds its tables in
-    ``__init__`` and supplies ``_workspace(opt, rows)`` and ``_launch(bu, bi, bj, batch, first, n_steps, apply)``."""
-    DEFAULT_OPTIMIZER = 'sgd'                   # config['optimizer'] == 'default'
-    DEFAULT_INIT = 'normal'                     # config['init_method'] == 'default'
+class DeviceRecommender(AbstractRecommender):
+    """What every GPU-path model shares, trained or not: the device set-up of the reference's GeneralRecommender
+    (AbstractRecommender.py:96-101), the multi-GPU policy, the caller-id range checks and the test-loader decoder."""
     MULTI_GPU = '{} runs as independent replicas only (DESIGN.md, multi-GPU section)'   # None: the class shards under torchrun
-    LOSS_TYPE = None                            # a fixed, unregularised loss: loss_type, reg_1 and reg_2 are not read
-    PARAMS = ('embed_user.weight', 'embed_item.weight')     # parameters() in order; attribute paths
-    BUFFERS = ()                                # in state_dict() after PARAMS, not in parameters()
-    STRICT_STATE = True                         # load_state_dict: every key of state_dict() must be given
-    SCRATCH_KEY = None                          # config key of the row count of a batch-sized scratch (built at first step)
 
     def __init__(self, config):
         super().__init__()
@@ -203,17 +196,70 @@ class GeneralRecommender(AbstractRecommender):
         self.device = torch.device('cuda', local if local < torch.cuda.device_count() else 0)
         torch.cuda.set_device(self.device)
         self.logger = config['logger']
-        self.steps_per_launch = int(config.get('steps_per_launch', 0))   # 0 = whole epoch in one launch
-        self.show_progress = bool(config.get('progress', True))
-        # 'torch' (default): the DataLoader's own CPU permutation -> the reference's batches bit for bit;
-        # 'device': torch.randperm on the GPU seeded from the global RNG (same distribution, no 8-byte/triple H2D)
-        self.shuffle_engine = str(config.get('shuffle_engine', DEFAULT_SHUFFLE_ENGINE))
         # one process per GPU (torchrun): user-sharded training / ranking, see daisyrec_b200/parallel.py
         import torch.distributed as dist
         self.world = dist.get_world_size() if dist.is_available() and dist.is_initialized() else 1
         self.rank_id = dist.get_rank() if self.world > 1 else 0
         if self.world > 1 and self.MULTI_GPU is not None:
             raise NotImplementedError(self.MULTI_GPU.format(type(self).__name__))
+
+    # ------------------------------------------------------------------ caller ids
+    def _check_ids(self, cols, bounds, names):
+        """nn.Embedding's IndexError when a column of caller ids leaves [0, bounds[c]): the kernels index raw tables.  Host
+        columns are checked on the host (no device sync), device columns in one ops.check_index_range launch."""
+        dev = []
+        for ids, hi, what in zip(cols, bounds, names):
+            t = torch.as_tensor(ids)
+            if t.is_cuda:
+                dev.append((t.reshape(-1).to(torch.int64), hi, what))
+            elif t.numel():
+                h = t.reshape(-1).to(torch.int64)
+                bad = int(((h < 0) | (h >= hi)).sum())
+                if bad:
+                    raise IndexError(f"index out of range in self: {bad} {what} id(s) outside [0, {int(hi)})")
+        if dev:
+            ids, bounds, names = zip(*dev)
+            ops.check_index_range(torch.stack(ids, 1).contiguous(), bounds, names)
+
+    def _rank_inputs(self, test_loader):
+        """The test loader's (users int64 [n], candidates int64 [n, C], topk) on the host, range-checked; None when it is
+        empty.  Reads ``dataset.data`` of a CandidatesDataset loader in bulk, else iterates (us, cands_ids) batches."""
+        data = getattr(getattr(test_loader, 'dataset', None), 'data', None)
+        if isinstance(data, (list, tuple)) and len(data) and len(data[0]) == 2:
+            users = np.fromiter((int(r[0]) for r in data), np.int64, len(data))
+            cands = np.stack([np.asarray(r[1], dtype=np.int64) for r in data])
+        else:
+            us, cs = [], []
+            for b_us, b_c in test_loader:
+                us.append(torch.as_tensor(b_us).reshape(-1).to(torch.int64))
+                cs.append(torch.as_tensor(b_c).to(torch.int64).reshape(us[-1].numel(), -1))
+            if not us:
+                return None
+            users, cands = torch.cat(us).numpy(), torch.cat(cs).numpy()
+        if len(users) == 0:
+            return None
+        self._check_ids((users, cands), (self.user_num, self.item_num), ('test user', 'candidate item'))
+        return users, np.ascontiguousarray(cands), min(self.topk, cands.shape[1])
+
+
+class GeneralRecommender(DeviceRecommender):
+    """Shared plumbing of the trained GPU-path models.  A subclass declares its defaults and state as class data, builds its
+    tables in ``__init__`` and supplies ``_workspace(opt, rows)`` and ``_launch(bu, bi, bj, batch, first, n_steps, apply)``."""
+    DEFAULT_OPTIMIZER = 'sgd'                   # config['optimizer'] == 'default'
+    DEFAULT_INIT = 'normal'                     # config['init_method'] == 'default'
+    LOSS_TYPE = None                            # a fixed, unregularised loss: loss_type, reg_1 and reg_2 are not read
+    PARAMS = ('embed_user.weight', 'embed_item.weight')     # parameters() in order; attribute paths
+    BUFFERS = ()                                # in state_dict() after PARAMS, not in parameters()
+    STRICT_STATE = True                         # load_state_dict: every key of state_dict() must be given
+    SCRATCH_KEY = None                          # config key of the row count of a batch-sized scratch (built at first step)
+
+    def __init__(self, config):
+        super().__init__(config)
+        self.steps_per_launch = int(config.get('steps_per_launch', 0))   # 0 = whole epoch in one launch
+        self.show_progress = bool(config.get('progress', True))
+        # 'torch' (default): the DataLoader's own CPU permutation -> the reference's batches bit for bit;
+        # 'device': torch.randperm on the GPU seeded from the global RNG (same distribution, no 8-byte/triple H2D)
+        self.shuffle_engine = str(config.get('shuffle_engine', DEFAULT_SHUFFLE_ENGINE))
         # the reference's common keys (e.g. MFRecommender.py:46-59)
         self.lr, self.epochs, self.topk = config['lr'], config['epochs'], config['topk']
         self.user_num, self.item_num, self.factors = config['user_num'], config['item_num'], config['factors']
@@ -304,23 +350,6 @@ class GeneralRecommender(AbstractRecommender):
             self.train(was)
 
     # ------------------------------------------------------------------ caller ids
-    def _check_ids(self, cols, bounds, names):
-        """nn.Embedding's IndexError when a column of caller ids leaves [0, bounds[c]): the kernels index raw tables.  Host
-        columns are checked on the host (no device sync), device columns in one ops.check_index_range launch."""
-        dev = []
-        for ids, hi, what in zip(cols, bounds, names):
-            t = torch.as_tensor(ids)
-            if t.is_cuda:
-                dev.append((t.reshape(-1).to(torch.int64), hi, what))
-            elif t.numel():
-                h = t.reshape(-1).to(torch.int64)
-                bad = int(((h < 0) | (h >= hi)).sum())
-                if bad:
-                    raise IndexError(f"index out of range in self: {bad} {what} id(s) outside [0, {int(hi)})")
-        if dev:
-            ids, bounds, names = zip(*dev)
-            ops.check_index_range(torch.stack(ids, 1).contiguous(), bounds, names)
-
     def _device_ids(self, cols, bounds, names, dtype=torch.int32):
         """Range-checked caller ids -> one contiguous 1-D device tensor of ``dtype`` per column."""
         self._check_ids(cols, bounds, names)
@@ -333,26 +362,6 @@ class GeneralRecommender(AbstractRecommender):
         return self._device_ids((user, item), (self.user_num, self.item_num), ('user', 'item'), dtype)
 
     # ------------------------------------------------------------------ ranking
-    def _rank_inputs(self, test_loader):
-        """The test loader's (users int64 [n], candidates int64 [n, C], topk) on the host, range-checked; None when it is
-        empty.  Reads ``dataset.data`` of a CandidatesDataset loader in bulk, else iterates (us, cands_ids) batches."""
-        data = getattr(getattr(test_loader, 'dataset', None), 'data', None)
-        if isinstance(data, (list, tuple)) and len(data) and len(data[0]) == 2:
-            users = np.fromiter((int(r[0]) for r in data), np.int64, len(data))
-            cands = np.stack([np.asarray(r[1], dtype=np.int64) for r in data])
-        else:
-            us, cs = [], []
-            for b_us, b_c in test_loader:
-                us.append(torch.as_tensor(b_us).reshape(-1).to(torch.int64))
-                cs.append(torch.as_tensor(b_c).to(torch.int64).reshape(us[-1].numel(), -1))
-            if not us:
-                return None
-            users, cands = torch.cat(us).numpy(), torch.cat(cs).numpy()
-        if len(users) == 0:
-            return None
-        self._check_ids((users, cands), (self.user_num, self.item_num), ('test user', 'candidate item'))
-        return users, np.ascontiguousarray(cands), min(self.topk, cands.shape[1])
-
     def _dot_tables(self):
         """(P, Q) of the dot-product scorers (MF's rank kernels)."""
         return self.embed_user.weight, self.embed_item.weight

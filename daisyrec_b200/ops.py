@@ -819,3 +819,90 @@ def gemm_test(variant, dtype, A, B, C_out, M, N, K, bias=None, ref=None):
                                   C_out.stride(0), None if bias is None else _ptr(bias), None if ref is None else _ptr(ref),
                                   0 if ref is None else ref.stride(0), _stream()))
     return C_out
+
+
+# ------------------------------------------------------------------ EASE
+class EaseX:
+    """X of EASERecommender.fit on the device: CSR (row_ptr int64 [U+1], col int32 [nnz], val float32 [nnz]) and the exact-Gram
+    scale s (x 2^s are s8 integers), or -1 for the fp64 Gram."""
+
+    def __init__(self, row_ptr, col, val, scale, user_num, item_num):
+        self.row_ptr, self.col, self.val, self.scale = row_ptr, col, val, scale
+        self.user_num, self.item_num = user_num, item_num
+
+
+def ease_csr(d_u, d_i, d_v, user_num, item_num):
+    """COO (int32 users, int32 items, float64 values) on the device -> EaseX: duplicates summed in fp64 in row order, then
+    rounded once to fp32, as csr_matrix((values, (u, i))).astype(float32)."""
+    _dev(d_v, torch.float64, "values")
+    row_ptr, col = csr_build(d_u, d_i, user_num, item_num)
+    seq_ptr, _, order = skipgram_group(d_u, user_num, 0)
+    nnz = col.numel()
+    val = torch.empty(max(nnz, 1), dtype=torch.float32, device=d_u.device)
+    ws = torch.empty(L.lib().drb_ease_csr_workspace_bytes(item_num, nnz), dtype=torch.uint8, device=d_u.device)
+    scale = C.c_int32(0)
+    L.check(L.lib().drb_ease_csr(_ptr(seq_ptr), _ptr(order), _ptr(d_i), _ptr(d_v), user_num, item_num, _ptr(row_ptr), _ptr(col),
+                                 nnz, _ptr(ws), _ptr(val), C.byref(scale), _stream()))
+    return EaseX(row_ptr, col.contiguous(), val[:nnz], int(scale.value), user_num, item_num)
+
+
+def ease_workspace(X, scale=None):
+    """Scratch of ease_gram / ease_inverse / ease_weights (the Gram's user-chunk image is sized by the path: X.scale or ``scale``)."""
+    s = X.scale if scale is None else scale
+    return torch.empty(L.lib().drb_ease_workspace_bytes(X.user_num, X.item_num, s), dtype=torch.uint8, device=X.val.device)
+
+
+def ease_gram(X, reg, ws, out=None, scale=None):
+    """G = X^T X + reg I, fp64 [I, I]: s8 tensor cores when X.scale >= 0 (exact), else fp64 DMMA.  ``scale`` = -1 forces the
+    fp64 path (ws must have been sized for it)."""
+    s = X.scale if scale is None else scale
+    n = X.item_num
+    G = torch.empty((n, n), dtype=torch.float64, device=X.val.device) if out is None else _dev(out, torch.float64, "G")
+    L.check(L.lib().drb_ease_gram(_ptr(X.row_ptr), _ptr(X.col), _ptr(X.val), X.user_num, n, s, float(reg), _ptr(ws), _ptr(G),
+                                  _stream()))
+    return G
+
+
+def ease_inverse(G, ws):
+    """In place: G -> G^-1 (blocked sweep on DMMA).  numpy.linalg.LinAlgError when G is not positive definite."""
+    _dev(G, torch.float64, "G")
+    L.check(L.lib().drb_ease_inverse(_ptr(G), G.shape[0], _ptr(ws), _stream()))
+    return G
+
+
+def ease_weights(P, ws):
+    """In place: P -> B = -P / diag(P) (column j divided by P_jj), zero diagonal."""
+    _dev(P, torch.float64, "P")
+    L.check(L.lib().drb_ease_weights(_ptr(P), P.shape[0], _ptr(ws), _stream()))
+    return P
+
+
+def ease_rank(B, X, users, cands, topk, scores=False):
+    """-> int64 [n, topk] candidate item ids by s_c = sum_i x_ui B[c, i] (and the fp64 [n, C] scores when ``scores``)."""
+    _dev(B, torch.float64, "B"); _dev(users, torch.int64, "users"); _dev(cands, torch.int64, "cands")
+    n, cnum = cands.shape
+    out = torch.empty((n, topk), dtype=torch.int64, device=B.device)
+    sc = torch.empty((n, cnum), dtype=torch.float64, device=B.device) if scores else None
+    L.check(L.lib().drb_ease_rank(_ptr(B), B.shape[0], _ptr(X.row_ptr), _ptr(X.col), _ptr(X.val), _ptr(users), n, _ptr(cands),
+                                  cnum, topk, _ptr(out), None if sc is None else _ptr(sc), _stream()))
+    return (out, sc) if scores else out
+
+
+def ease_full_rank(B, X, users, topk, scores=False):
+    """-> int64 [n, topk] item ids by s = x_u B (and the fp64 [n, I] scores when ``scores``)."""
+    _dev(B, torch.float64, "B"); _dev(users, torch.int64, "users")
+    n = users.numel()
+    out = torch.empty((n, topk), dtype=torch.int64, device=B.device)
+    sc = torch.empty((n, B.shape[0]), dtype=torch.float64, device=B.device)
+    L.check(L.lib().drb_ease_full_rank(_ptr(B), B.shape[0], _ptr(X.row_ptr), _ptr(X.col), _ptr(X.val), _ptr(users), n, topk,
+                                       _ptr(sc), _ptr(out), _stream()))
+    return (out, sc) if scores else out
+
+
+def ease_predict(B, X, users, items):
+    """-> fp64 [n]: x_u . B[:, i] per (u, i) pair."""
+    _dev(B, torch.float64, "B"); _dev(users, torch.int64, "users"); _dev(items, torch.int64, "items")
+    out = torch.empty(users.numel(), dtype=torch.float64, device=B.device)
+    L.check(L.lib().drb_ease_predict(_ptr(B), B.shape[0], _ptr(X.row_ptr), _ptr(X.col), _ptr(X.val), _ptr(users), _ptr(items),
+                                     users.numel(), _ptr(out), _stream()))
+    return out

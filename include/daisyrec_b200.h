@@ -38,6 +38,7 @@ extern "C" {
 #define DRB_ERR_EMPTY_SET 4   /* a user has no un-interacted item: numpy "a cannot be empty"      */
 #define DRB_ERR_NO_DEVICE 5   /* no sm_90 device / kernel image not loadable on this device     */
 #define DRB_ERR_PEER 6        /* multi-GPU peer exchange: a rank did not reach the rendezvous in time */
+#define DRB_ERR_NOT_PD 7      /* EASE: G + reg I has a pivot <= 0 (np.linalg.inv's LinAlgError)  */
 
 #define DRB_OPT_SGD 0         /* optim.SGD(lr)   AbstractRecommender.py:55-56                     */
 #define DRB_OPT_ADAM 1        /* optim.Adam(lr)  AbstractRecommender.py:53-54 (dense, torch defaults) */
@@ -510,6 +511,41 @@ int drb_csr_build(const int32_t *d_row, const int32_t *d_col, int64_t nnz, int32
 int drb_lgcn_build_adj(const int64_t *d_ui_ptr, const int32_t *d_ui_col, const int64_t *d_iu_ptr, const int32_t *d_iu_col,
                        int32_t user_num, int32_t item_num, int64_t nnz, int64_t *d_adj_ptr, int32_t *d_adj_col,
                        float *d_adj_val, void *stream);
+
+/* ---- EASE: daisy/model/EASERecommender.py (Steck 2019), csrc/ease.cu ----------------------------------------------------
+ * drb_ease_csr        X = csr_matrix((values, (u, i)), (U, I)).astype(float32) (EASERecommender.py:30-35): d_val[k] = the fp64
+ *                     sum, in row order, of the COO values of slot k of the drb_csr_build CSR (d_row_ptr, d_col), rounded once
+ *                     to fp32.  d_seq_ptr / d_order: the rows grouped by user in row order (drb_skipgram_group).
+ *                     *h_scale = smallest s in [0, 7] with every x 2^s an integer in [-127, 127] and
+ *                     max_i sum_u (x_ui 2^s)^2 < 2^31 (the exact Gram applies), else -1.  Synchronises.
+ * drb_ease_gram       G = X^T X + reg I (:37-39), fp64 [I, I] row-major; s8 tensor cores (exact) when scale >= 0, else fp64
+ *                     DMMA.  Bitwise reproducible; on the exact path the exact Gram, bitwise equal to scipy's
+ *                     fp32 product upcast to fp64 while max_i sum_u (x_ui 2^s)^2 < 2^24.
+ * drb_ease_inverse    P = G^-1 in place (np.linalg.inv, :42), blocked sweep operator on DMMA; DRB_ERR_NOT_PD when G is not
+ *                     positive definite.  Synchronises.
+ * drb_ease_weights    B = -P / diag(P) by column, zero diagonal, in place (:43-44).
+ * d_ws: drb_ease_workspace_bytes(U, I, scale) bytes, shared by gram / inverse / weights.
+ * drb_ease_rank       rank() (:53-70): s_c = sum_i x_ui B[cand_c, i] (rows of B), top-k by (score desc, candidate position
+ *                     asc) -> int64 item ids [n_users, topk]; d_scores (NULL or fp64 [n_users, cand_num]) receives s.
+ * drb_ease_full_rank  full_rank() (:72-74): s = x_u B over all items into d_scores fp64 [n_users, I], top-k by (score desc,
+ *                     item asc) -> int64 [n_users, topk].  No masking of train items.
+ * drb_ease_predict    predict() (:49-50): out[p] = x_{u_p} . B[:, i_p], fp64. */
+size_t drb_ease_csr_workspace_bytes(int32_t item_num, int64_t nnz);
+int drb_ease_csr(const int64_t *d_seq_ptr, const int32_t *d_order, const int32_t *d_coo_i, const double *d_coo_v, int32_t user_num,
+                 int32_t item_num, const int64_t *d_row_ptr, const int32_t *d_col, int64_t nnz, void *d_ws, float *d_val,
+                 int32_t *h_scale, void *stream);
+size_t drb_ease_workspace_bytes(int32_t user_num, int32_t item_num, int32_t scale);
+int drb_ease_gram(const int64_t *d_row_ptr, const int32_t *d_col, const float *d_val, int32_t user_num, int32_t item_num,
+                  int32_t scale, double reg, void *d_ws, double *d_G, void *stream);
+int drb_ease_inverse(double *d_G, int32_t item_num, void *d_ws, void *stream);
+int drb_ease_weights(double *d_P, int32_t item_num, void *d_ws, void *stream);
+int drb_ease_rank(const double *d_B, int32_t item_num, const int64_t *d_row_ptr, const int32_t *d_col, const float *d_val,
+                  const int64_t *d_users, int64_t n_users, const int64_t *d_cands, int32_t cand_num, int32_t topk, int64_t *d_out,
+                  double *d_scores, void *stream);
+int drb_ease_full_rank(const double *d_B, int32_t item_num, const int64_t *d_row_ptr, const int32_t *d_col, const float *d_val,
+                       const int64_t *d_users, int32_t n_users, int32_t topk, double *d_scores, int64_t *d_out, void *stream);
+int drb_ease_predict(const double *d_B, int32_t item_num, const int64_t *d_row_ptr, const int32_t *d_col, const float *d_val,
+                     const int64_t *d_users, const int64_t *d_items, int64_t n_pairs, double *d_out, void *stream);
 
 /* ---- evaluation: calc_ranking_results / Metric.run ------------------------------------------------
  * daisy/utils/metrics.py:18-57 (cut-off loop), :59-96 (dispatch), :98-251 (the KPIs).
