@@ -8,6 +8,7 @@
 //                     the smallest s in [0, 7] with every x 2^s an integer in [-127, 127] and max_i sum_u (x_ui 2^s)^2
 //                     < 2^31.  By Cauchy-Schwarz that bounds every |G_ij| and every partial sum, so s8 x s8 -> s32 cannot
 //                     overflow.
+//   drb_ease_scale    the same decision for a CSR whose values are already in place (ItemKNN's transformed copies of X).
 //   drb_ease_gram     G = X^T X + reg I, fp64 [n, n].  User chunks are expanded into a dense item-major image and the lower
 //                     triangle of tiles accumulates image * image^T:
 //                       exact path   s8 operands, s32 accumulation on the tensor cores (mma.sync m16n8k32), the chunk's
@@ -30,6 +31,7 @@
 
 #include "common.cuh"
 #include "dmma.cuh"
+#include "topk.cuh"
 
 namespace drb {
 
@@ -92,6 +94,31 @@ struct CsrStats {
 };
 
 // ---------------------------------------------------------------- X's values
+// one user's stored values [b, e) folded into the statistics the exact-Gram rule reads
+// (val is not __restrict__: ease_values_kernel has just written it)
+__device__ __forceinline__ void row_stats(const float *val, const int32_t *__restrict__ col, long long b, long long e,
+                                          double *__restrict__ colsq, CsrStats *__restrict__ st)
+{
+    unsigned smax = 0, amax = 0;
+    for (long long k = b; k < e; ++k) {
+        const float x = val[k];
+        unsigned s = 8;
+        if (isfinite(x)) {
+            for (unsigned t = 0; t < 8; ++t) {
+                const float y = ldexpf(x, (int)t);
+                if (y == floorf(y)) { s = t; break; }
+            }
+        }
+        smax = max(smax, s);
+        amax = max(amax, __float_as_uint(fabsf(x)));   // NaN compares above every finite value
+        atomicAdd(colsq + col[k], (double)x * (double)x);
+    }
+    if (e > b) {
+        atomicMax(&st->smax, smax);
+        atomicMax(&st->amax, amax);
+    }
+}
+
 // One thread per user walks the user's COO rows in row order (d_order: stable grouping) and adds each value into its CSR
 // slot: every slot's duplicates are summed in fp64 in row order, then rounded once to fp32.
 __global__ void ease_values_kernel(const int64_t *__restrict__ seq_ptr, const int32_t *__restrict__ order,
@@ -113,26 +140,17 @@ __global__ void ease_values_kernel(const int64_t *__restrict__ seq_ptr, const in
             }
             sum[lo] += coo_v[r];
         }
-        unsigned smax = 0, amax = 0;
-        for (long long k = b; k < e; ++k) {
-            const float x = (float)sum[k];
-            val[k] = x;
-            unsigned s = 8;
-            if (isfinite(x)) {
-                for (unsigned t = 0; t < 8; ++t) {
-                    const float y = ldexpf(x, (int)t);
-                    if (y == floorf(y)) { s = t; break; }
-                }
-            }
-            smax = max(smax, s);
-            amax = max(amax, __float_as_uint(fabsf(x)));   // NaN compares above every finite value
-            atomicAdd(colsq + col[k], (double)x * (double)x);
-        }
-        if (e > b) {
-            atomicMax(&st->smax, smax);
-            atomicMax(&st->amax, amax);
-        }
+        for (long long k = b; k < e; ++k) val[k] = (float)sum[k];
+        row_stats(val, col, b, e, colsq, st);
     }
+}
+
+// the statistics of a CSR whose values are already in place (a thread per user)
+__global__ void ease_stats_kernel(const int64_t *__restrict__ row_ptr, const int32_t *__restrict__ col,
+                                  const float *__restrict__ val, int U, double *__restrict__ colsq, CsrStats *__restrict__ st)
+{
+    for (int u = blockIdx.x * blockDim.x + threadIdx.x; u < U; u += gridDim.x * blockDim.x)
+        row_stats(val, col, row_ptr[u], row_ptr[u + 1], colsq, st);
 }
 
 __global__ void ease_sqmax_kernel(const double *__restrict__ colsq, int I, CsrStats *__restrict__ st)
@@ -406,67 +424,6 @@ __global__ void ease_weights_kernel(double *__restrict__ P, int n, const double 
 }
 
 // ---------------------------------------------------------------- scoring
-// 64-bit key ordered as the fp64 score (-0 counted as +0)
-__device__ __forceinline__ unsigned long long score_key(double s)
-{
-    if (s == 0.0) s = 0.0;
-    const unsigned long long b = (unsigned long long)__double_as_longlong(s);
-    return (b >> 63) ? ~b : (b | 0x8000000000000000ull);
-}
-
-__device__ __forceinline__ bool key_before(unsigned long long ka, int pa, unsigned long long kb, int pb)
-{
-    return ka > kb || (ka == kb && pa < pb);
-}
-
-// top-k of sc[0 .. C) by (score descending, position ascending): k rounds of a block arg-max over the elements after the
-// previous pick.  out[r] = ids ? ids[pos] : pos.
-__device__ void block_topk(const double *sc, int C, int k, const int64_t *ids, int64_t *out)
-{
-    __shared__ unsigned long long wk[32];
-    __shared__ int wp[32];
-    __shared__ unsigned long long s_lk;
-    __shared__ int s_lp;
-    const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5, nw = (blockDim.x + 31) >> 5;
-    unsigned long long lk = ~0ull;
-    int lp = -1;
-    for (int r = 0; r < k; ++r) {
-        unsigned long long bk = 0;
-        int bp = 0x7fffffff;
-        for (int c = tid; c < C; c += blockDim.x) {
-            const unsigned long long kc = score_key(sc[c]);
-            if (key_before(lk, lp, kc, c) && key_before(kc, c, bk, bp)) { bk = kc; bp = c; }
-        }
-#pragma unroll
-        for (int off = 16; off >= 1; off >>= 1) {
-            const unsigned long long ok = __shfl_xor_sync(0xffffffffu, bk, off);
-            const int op = __shfl_xor_sync(0xffffffffu, bp, off);
-            if (key_before(ok, op, bk, bp)) { bk = ok; bp = op; }
-        }
-        if (lane == 0) { wk[warp] = bk; wp[warp] = bp; }
-        __syncthreads();
-        if (warp == 0) {
-            bk = lane < nw ? wk[lane] : 0ull;
-            bp = lane < nw ? wp[lane] : 0x7fffffff;
-#pragma unroll
-            for (int off = 16; off >= 1; off >>= 1) {
-                const unsigned long long ok = __shfl_xor_sync(0xffffffffu, bk, off);
-                const int op = __shfl_xor_sync(0xffffffffu, bp, off);
-                if (key_before(ok, op, bk, bp)) { bk = ok; bp = op; }
-            }
-            if (lane == 0) {
-                s_lk = bk;
-                s_lp = bp;
-                out[r] = ids ? ids[bp] : (int64_t)bp;
-            }
-        }
-        __syncthreads();
-        lk = s_lk;
-        lp = s_lp;
-        __syncthreads();
-    }
-}
-
 constexpr int kRankThreads = 256;
 
 // one CTA per test user: s_c = sum_{i in row(u)} x_ui B[cand_c, i] (warp per candidate), then top-k of the C scores
@@ -527,6 +484,27 @@ __global__ void ease_predict_kernel(const double *__restrict__ B, int n, const i
     }
 }
 
+// the exact-Gram rule on the gathered statistics (drb_ease_csr's comment above); synchronises
+static int exact_scale(const double *colsq, int item_num, CsrStats *stats, int32_t *h_scale, cudaStream_t st)
+{
+    ease_sqmax_kernel<<<grid_for(item_num, 256), 256, 0, st>>>(colsq, item_num, stats);
+    DRB_CUDA(cudaGetLastError());
+    CsrStats h;
+    DRB_CUDA(cudaMemcpyAsync(&h, stats, sizeof(h), cudaMemcpyDeviceToHost, st));
+    DRB_CUDA(cudaStreamSynchronize(st));
+    int s = -1;
+    if (h.smax <= 7) {
+        uint32_t a = h.amax;
+        float amax;
+        memcpy(&amax, &a, sizeof(amax));
+        double sq;
+        memcpy(&sq, &h.sqmax, sizeof(sq));
+        if ((double)amax * (double)(1 << h.smax) <= 127.0 && sq * (double)(1 << (2 * h.smax)) < 2147483648.0) s = (int)h.smax;
+    }
+    *h_scale = s;
+    return DRB_OK;
+}
+
 }  // namespace drb
 
 using namespace drb;
@@ -551,22 +529,19 @@ extern "C" int drb_ease_csr(const int64_t *d_seq_ptr, const int32_t *d_order, co
     DRB_CUDA(cudaMemsetAsync(d_ws, 0, 256 + sizeof(double) * (size_t)item_num, st));
     ease_values_kernel<<<grid_for(user_num, 128), 128, 0, st>>>(d_seq_ptr, d_order, d_coo_i, d_coo_v, user_num, d_row_ptr, d_col,
                                                                  sum, d_val, colsq, stats);
-    ease_sqmax_kernel<<<grid_for(item_num, 256), 256, 0, st>>>(colsq, item_num, stats);
-    DRB_CUDA(cudaGetLastError());
-    CsrStats h;
-    DRB_CUDA(cudaMemcpyAsync(&h, stats, sizeof(h), cudaMemcpyDeviceToHost, st));
-    DRB_CUDA(cudaStreamSynchronize(st));
-    int s = -1;
-    if (h.smax <= 7) {
-        uint32_t a = h.amax;
-        float amax;
-        memcpy(&amax, &a, sizeof(amax));
-        double sq;
-        memcpy(&sq, &h.sqmax, sizeof(sq));
-        if ((double)amax * (double)(1 << h.smax) <= 127.0 && sq * (double)(1 << (2 * h.smax)) < 2147483648.0) s = (int)h.smax;
-    }
-    *h_scale = s;
-    return DRB_OK;
+    return exact_scale(colsq, item_num, stats, h_scale, st);
+}
+
+extern "C" int drb_ease_scale(const int64_t *d_row_ptr, const int32_t *d_col, const float *d_val, int32_t user_num,
+                              int32_t item_num, void *d_ws, int32_t *h_scale, void *stream)
+{
+    DRB_REQUIRE(d_row_ptr && d_ws && h_scale && user_num > 0 && item_num > 0, "ease_scale: bad arguments");
+    cudaStream_t st = (cudaStream_t)stream;
+    CsrStats *stats = (CsrStats *)d_ws;
+    double *colsq = (double *)((char *)d_ws + 256);
+    DRB_CUDA(cudaMemsetAsync(d_ws, 0, 256 + sizeof(double) * (size_t)item_num, st));
+    ease_stats_kernel<<<grid_for(user_num, 128), 128, 0, st>>>(d_row_ptr, d_col, d_val, user_num, colsq, stats);
+    return exact_scale(colsq, item_num, stats, h_scale, st);
 }
 
 extern "C" size_t drb_ease_workspace_bytes(int32_t user_num, int32_t item_num, int32_t scale)

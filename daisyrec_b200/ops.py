@@ -906,3 +906,88 @@ def ease_predict(B, X, users, items):
     L.check(L.lib().drb_ease_predict(_ptr(B), B.shape[0], _ptr(X.row_ptr), _ptr(X.col), _ptr(X.val), _ptr(users), _ptr(items),
                                      users.numel(), _ptr(out), _stream()))
     return out
+
+
+# ------------------------------------------------------------------ ItemKNN
+# similarity -> (value transform, formula family, ss is the root of the sum of squares): csrc/itemknn.cu.  asymmetric with the
+# class's fixed alpha = 0.5 raises ss to the power 1.0 on both sides, which is cosine.
+KNN_SIMILARITY = {'cosine': (0, 0, 1), 'asymmetric': (0, 0, 1), 'adjusted': (1, 0, 1), 'pearson': (2, 0, 1),
+                  'jaccard': (3, 1, 0), 'tanimoto': (3, 1, 0), 'dice': (3, 2, 0), 'tversky': (3, 3, 0)}
+
+
+class KnnNeighbours:
+    """W of ItemKNNCF by column: idx int32 [I, maxk] (ascending ids, -1 past the count), val float32 [I, maxk], cnt int32 [I]."""
+
+    def __init__(self, idx, val, cnt):
+        self.idx, self.val, self.cnt = idx, val, cnt
+        self.maxk = idx.shape[1]
+
+
+def itemknn_transform(X, similarity):
+    """The similarity's view of X (KNNCFRecommender.py:165-233, 257-261) -> (EaseX of the transformed values with its own
+    exact-Gram scale, ss float32 [I], item_ptr int64 [I+1] of the stored entries per item).  X itself is left as it is."""
+    transform, _, root = KNN_SIMILARITY[similarity]
+    dev, nnz = X.val.device, X.col.numel()
+    item_ptr, _, order = skipgram_group(X.col, X.item_num, 0)
+    val = torch.empty(max(nnz, 1), dtype=torch.float32, device=dev)
+    ss = torch.empty(X.item_num, dtype=torch.float32, device=dev)
+    L.check(L.lib().drb_itemknn_transform(_ptr(X.row_ptr), _ptr(X.val), X.user_num, X.item_num, _ptr(item_ptr), _ptr(order),
+                                          transform, root, _ptr(val), _ptr(ss), _stream()))
+    ws = torch.empty(L.lib().drb_ease_csr_workspace_bytes(X.item_num, 0), dtype=torch.uint8, device=dev)
+    scale = C.c_int32(0)
+    L.check(L.lib().drb_ease_scale(_ptr(X.row_ptr), _ptr(X.col), _ptr(val), X.user_num, X.item_num, _ptr(ws), C.byref(scale),
+                                   _stream()))
+    return EaseX(X.row_ptr, X.col, val[:nnz], int(scale.value), X.user_num, X.item_num), ss, item_ptr
+
+
+def itemknn_neighbours(G, ss, similarity, normalize, shrink, maxk):
+    """compute_similarity's column loop (:302-356) on the Gram matrix G fp64 [n, n] of the transformed values ->
+    KnnNeighbours.  Per column the min(maxk, n) largest weights by (weight descending, id ascending), exact zeros dropped."""
+    _dev(G, torch.float64, "G"); _dev(ss, torch.float32, "ss")
+    n = G.shape[0]
+    idx = torch.empty((n, maxk), dtype=torch.int32, device=G.device)
+    val = torch.empty((n, maxk), dtype=torch.float32, device=G.device)
+    cnt = torch.empty(n, dtype=torch.int32, device=G.device)
+    L.check(L.lib().drb_itemknn_neighbours(_ptr(G), n, _ptr(ss), KNN_SIMILARITY[similarity][1], int(bool(normalize)),
+                                           float(np.float32(shrink)), maxk, _ptr(idx), _ptr(val), _ptr(cnt), _stream()))
+    return KnnNeighbours(idx, val, cnt)
+
+
+def itemknn_scores(X, W, users, cands=None):
+    """pred_mat[u, c] = sum_{i in N(c)} x_ui W[i, c] in fp64 over ascending i -> [n, C] for ``cands`` int64 [n, C], or
+    [n, I] over every item."""
+    _dev(users, torch.int64, "users")
+    n = users.numel()
+    cnum = X.item_num if cands is None else _dev(cands, torch.int64, "cands").shape[1]
+    sc = torch.empty((n, cnum), dtype=torch.float64, device=users.device)
+    L.check(L.lib().drb_itemknn_scores(_ptr(X.row_ptr), _ptr(X.col), _ptr(X.val), _ptr(W.idx), _ptr(W.val), _ptr(W.cnt), W.maxk,
+                                       X.item_num, _ptr(users), n, None if cands is None else _ptr(cands), cnum, _ptr(sc),
+                                       _stream()))
+    return sc
+
+
+def _itemknn_topk(sc, cands, topk):
+    out = torch.empty((sc.shape[0], topk), dtype=torch.int64, device=sc.device)
+    L.check(L.lib().drb_itemknn_topk(_ptr(sc), sc.shape[0], sc.shape[1], None if cands is None else _ptr(cands), topk, _ptr(out),
+                                     _stream()))
+    return out
+
+
+def itemknn_rank(X, W, users, cands, topk, scores=False):
+    """-> int64 [n, topk] candidate ids by (score descending, candidate position ascending) (and the scores when asked)."""
+    sc = itemknn_scores(X, W, users, cands)
+    out = _itemknn_topk(sc, cands, topk)
+    return (out, sc) if scores else out
+
+
+def itemknn_full_rank(X, W, users, topk, scores=False):
+    """-> int64 [n, topk] item ids by (score descending, id ascending) over every item (and the scores when asked)."""
+    sc = itemknn_scores(X, W, users)
+    out = _itemknn_topk(sc, None, topk)
+    return (out, sc) if scores else out
+
+
+def itemknn_predict(X, W, users, items):
+    """-> fp64 [n]: pred_mat[u, i] per (u, i) pair."""
+    _dev(items, torch.int64, "items")
+    return itemknn_scores(X, W, users, items.reshape(-1, 1)).reshape(-1)

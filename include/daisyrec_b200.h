@@ -547,6 +547,38 @@ int drb_ease_full_rank(const double *d_B, int32_t item_num, const int64_t *d_row
 int drb_ease_predict(const double *d_B, int32_t item_num, const int64_t *d_row_ptr, const int32_t *d_col, const float *d_val,
                      const int64_t *d_users, const int64_t *d_items, int64_t n_pairs, double *d_out, void *stream);
 
+/* ---- ItemKNN: daisy/model/KNNCFRecommender.py (ItemKNNCF / Similarity), csrc/itemknn.cu ---------------------------------
+ * drb_ease_scale          the exact-Gram scale of drb_ease_csr for a CSR whose fp32 values are in place; d_ws as for
+ *                         drb_ease_csr (drb_ease_csr_workspace_bytes).  Synchronises.
+ * drb_itemknn_transform   d_val_out = the similarity's view of X (:165-233): transform 0 the values as they are, 1 minus the
+ *                         user's mean (adjusted), 2 minus the item's mean (pearson), 3 every stored value 1 (jaccard, tanimoto,
+ *                         dice, tversky); d_ss[i] = fp32 sum of the squared transformed values of item i (:257), its square root
+ *                         when root != 0 (:261).  d_item_ptr int64 [I+1] / d_item_order int32 [nnz]: the CSR slots grouped by
+ *                         item, users ascending (drb_skipgram_group on the CSR's column ids).  fp32 sums in ascending order.
+ * drb_itemknn_neighbours  compute_similarity's loop (:302-356) from the Gram matrix d_G fp64 [n, n] of the transformed values:
+ *                         for column j, w_i = f(G_ij, ss_i, ss_j) in fp32, w_j = 0, the min(maxk, n) largest by (weight
+ *                         descending, id ascending), exact zeros dropped.  family 0 cosine / adjusted / pearson / asymmetric
+ *                         (alpha 0.5) with normalize and shrink as the reference, 1 tanimoto / jaccard, 2 dice, 3 tversky
+ *                         (alpha = beta = 1).  Out, per column and by ascending id: d_nbr_idx int32 [n, maxk] (-1 past the
+ *                         count), d_nbr_val fp32 [n, maxk], d_nbr_cnt int32 [n].  maxk in [1, 1024].  Bitwise reproducible.
+ * drb_itemknn_scores      pred_mat[u, c] = sum_{i in N(c)} x_ui W[i, c] (:432) for each row's user and candidates (d_cands
+ *                         int64 [n_rows, cand_num], or NULL with cand_num = item_num for every item), fp64, ascending i, no
+ *                         FMA -> d_scores fp64 [n_rows, cand_num].
+ * drb_itemknn_topk        top-k of each score row by (score desc, position asc) -> int64 [n_rows, topk]: the candidate ids,
+ *                         or the positions when d_cands is NULL. */
+int drb_ease_scale(const int64_t *d_row_ptr, const int32_t *d_col, const float *d_val, int32_t user_num, int32_t item_num,
+                   void *d_ws, int32_t *h_scale, void *stream);
+int drb_itemknn_transform(const int64_t *d_row_ptr, const float *d_val_in, int32_t user_num, int32_t item_num,
+                          const int64_t *d_item_ptr, const int32_t *d_item_order, int32_t transform, int32_t root,
+                          float *d_val_out, float *d_ss, void *stream);
+int drb_itemknn_neighbours(const double *d_G, int32_t n, const float *d_ss, int32_t family, int32_t normalize, float shrink,
+                           int32_t maxk, int32_t *d_nbr_idx, float *d_nbr_val, int32_t *d_nbr_cnt, void *stream);
+int drb_itemknn_scores(const int64_t *d_row_ptr, const int32_t *d_col, const float *d_val, const int32_t *d_nbr_idx,
+                       const float *d_nbr_val, const int32_t *d_nbr_cnt, int32_t maxk, int32_t item_num, const int64_t *d_users,
+                       int64_t n_rows, const int64_t *d_cands, int32_t cand_num, double *d_scores, void *stream);
+int drb_itemknn_topk(const double *d_scores, int64_t n_rows, int32_t cand_num, const int64_t *d_cands, int32_t topk,
+                     int64_t *d_out, void *stream);
+
 /* ---- evaluation: calc_ranking_results / Metric.run ------------------------------------------------
  * daisy/utils/metrics.py:18-57 (cut-off loop), :59-96 (dispatch), :98-251 (the KPIs).
  * d_preds: rank()'s float32 [n_users, ld] output; ground truth as CSR aligned with its rows
