@@ -178,6 +178,11 @@ SIGNATURES = {
     "drb_itemknn_neighbours": (C.c_int, [vp, C.c_int32, vp, C.c_int32, C.c_int32, C.c_float, C.c_int32, vp, vp, vp, vp]),
     "drb_itemknn_scores": (C.c_int, [vp, vp, vp, vp, vp, vp, C.c_int32, C.c_int32, vp, C.c_int64, vp, C.c_int32, vp, vp]),
     "drb_itemknn_topk": (C.c_int, [vp, C.c_int64, C.c_int32, vp, C.c_int32, vp, vp]),
+    "drb_slim_workspace_bytes": (C.c_size_t, [C.c_int32, C.c_int32]),
+    "drb_slim_live": (C.c_int, [vp, C.c_int32, C.c_int32, C.c_int32, C.c_double, C.c_int32, vp, vp, vp, vp, vp, vp]),
+    "drb_slim_solve": (C.c_int, [vp, C.c_int32, C.c_int32, C.c_int32, C.c_double, C.c_double, C.c_double, C.c_int32,
+                                 vp, vp, vp, vp, vp, vp, vp, vp, vp]),
+    "drb_slim_select": (C.c_int, [vp, vp, vp, C.c_int32, C.c_int32, C.c_int32, C.c_int32, vp, vp, vp, vp]),
     "drb_rank_metrics_workspace_bytes": (C.c_size_t, [C.c_int32, C.c_int32]),
     "drb_rank_metrics": (C.c_int, [vp, C.c_int64, C.c_int32, vp, vp, vp, C.c_int32, C.c_int32, vp, vp, vp, vp]),
     "drb_rank_metrics_host": (C.c_int, [vp, C.c_int64, C.c_int32, vp, vp, vp, C.c_int32, C.c_int32, vp, vp]),

@@ -242,6 +242,52 @@ class DeviceRecommender(AbstractRecommender):
         return users, np.ascontiguousarray(cands), min(self.topk, cands.shape[1])
 
 
+class NeighbourScorer(DeviceRecommender):
+    """The item-item models whose prediction is X W with W kept as at most ``maxk`` neighbours per item (ops.KnnNeighbours):
+    ItemKNNCF and SLiM.  Subclasses set ``self._X`` (ops.EaseX), ``self._W`` and ``self._w_host = None`` in ``fit``.  Entries of
+    X W are summed on demand in fp64 over ascending neighbour ids, the order scipy's product adds in; the product itself is not
+    materialised."""
+
+    def _neighbour_csc(self):
+        """W as scipy csc_matrix float32 [I, I], column c holding the neighbours of item c (None before fit)."""
+        if self._W is None:
+            return None
+        import scipy.sparse as sp
+        cnt = self._W.cnt.cpu().numpy().astype(np.int64)
+        keep = np.arange(self._W.maxk)[None, :] < cnt[:, None]
+        return sp.csc_matrix((self._W.val.cpu().numpy()[keep], self._W.idx.cpu().numpy()[keep],
+                              np.concatenate([[0], np.cumsum(cnt)])), shape=(self.item_num, self.item_num))
+
+    def _predict_score(self, u, i):
+        us, its = self._ids((u,), (i,))
+        return np.float64(ops.itemknn_predict(self._X, self._W, us, its).item())
+
+    def rank(self, test_loader):
+        """-> int64 ndarray [n_test_users, topk] of candidate ids by (X W)[u, c], ties by candidate position; None for an empty
+        loader."""
+        ins = self._rank_inputs(test_loader)
+        if ins is None:
+            return None
+        users, cands, k = ins
+        self._ids(())
+        return ops.itemknn_rank(self._X, self._W, torch.from_numpy(users).to(self.device),
+                                torch.from_numpy(cands).to(self.device), k).cpu().numpy()
+
+    def full_rank(self, u):
+        """-> int64 ndarray [topk] of the top items of user u; no masking of train items."""
+        users = self._ids((u,))[0]
+        return ops.itemknn_full_rank(self._X, self._W, users, min(self.topk, self.item_num))[0].cpu().numpy()
+
+    def _ids(self, users, items=None):
+        if self._W is None:
+            raise RuntimeError(f'{type(self).__name__}: fit() must run before scoring')
+        cols, bounds, names = [users], [self.user_num], ['user']
+        if items is not None:
+            cols, bounds, names = cols + [items], bounds + [self.item_num], names + ['item']
+        self._check_ids(cols, bounds, names)
+        return [torch.as_tensor(np.asarray(c, dtype=np.int64)).reshape(-1).to(self.device) for c in cols]
+
+
 class GeneralRecommender(DeviceRecommender):
     """Shared plumbing of the trained GPU-path models.  A subclass declares its defaults and state as class data, builds its
     tables in ``__init__`` and supplies ``_workspace(opt, rows)`` and ``_launch(bu, bi, bj, batch, first, n_steps, apply)``."""

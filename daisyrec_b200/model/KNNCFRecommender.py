@@ -20,10 +20,10 @@ import scipy.sparse as sp
 import torch
 
 from .. import ops
-from .AbstractRecommender import DeviceRecommender
+from .AbstractRecommender import NeighbourScorer
 
 
-class ItemKNNCF(DeviceRecommender):
+class ItemKNNCF(NeighbourScorer):
     MULTI_GPU = '{} runs on a single GPU'
 
     def __init__(self, config):
@@ -89,11 +89,8 @@ class ItemKNNCF(DeviceRecommender):
     def w_sparse(self):
         """W as the reference builds it: scipy csc_matrix float32 [I, I], column c holding the neighbours of item c (built on
         first use)."""
-        if self._w_host is None and self._W is not None:
-            cnt = self._W.cnt.cpu().numpy().astype(np.int64)
-            keep = np.arange(self._W.maxk)[None, :] < cnt[:, None]
-            self._w_host = sp.csc_matrix((self._W.val.cpu().numpy()[keep], self._W.idx.cpu().numpy()[keep],
-                                          np.concatenate([[0], np.cumsum(cnt)])), shape=(self.item_num, self.item_num))
+        if self._w_host is None:
+            self._w_host = self._neighbour_csc()
         return self._w_host
 
     # ------------------------------------------------------------------ scoring
@@ -101,30 +98,13 @@ class ItemKNNCF(DeviceRecommender):
         """-> numpy.float64: pred_mat[u, i] (KNNCFRecommender.py:434-438)."""
         if u >= self.user_num or i >= self.item_num:
             raise ValueError('User and/or item is unkown.')
-        us, its = self._ids((u,), (i,))
-        return np.float64(ops.itemknn_predict(self._X, self._W, us, its).item())
+        return self._predict_score(u, i)
 
     def rank(self, test_loader):
         """-> int64 ndarray [n_test_users, topk] of candidate ids by pred_mat[u, c], ties by candidate position
         (KNNCFRecommender.py:440-452)."""
-        ins = self._rank_inputs(test_loader)
-        if ins is None:
-            return None
-        users, cands, k = ins
-        self._ids(())
-        return ops.itemknn_rank(self._X, self._W, torch.from_numpy(users).to(self.device),
-                                torch.from_numpy(cands).to(self.device), k).cpu().numpy()
+        return super().rank(test_loader)
 
     def full_rank(self, u):
         """-> int64 ndarray [topk] of the top items of user u; no masking of train items (KNNCFRecommender.py:454-457)."""
-        users = self._ids((u,))[0]
-        return ops.itemknn_full_rank(self._X, self._W, users, min(self.topk, self.item_num))[0].cpu().numpy()
-
-    def _ids(self, users, items=None):
-        if self._W is None:
-            raise RuntimeError('ItemKNNCF: fit() must run before scoring')
-        cols, bounds, names = [users], [self.user_num], ['user']
-        if items is not None:
-            cols, bounds, names = cols + [items], bounds + [self.item_num], names + ['item']
-        self._check_ids(cols, bounds, names)
-        return [torch.as_tensor(np.asarray(c, dtype=np.int64)).reshape(-1).to(self.device) for c in cols]
+        return super().full_rank(u)

@@ -991,3 +991,72 @@ def itemknn_predict(X, W, users, items):
     """-> fp64 [n]: pred_mat[u, i] per (u, i) pair."""
     _dev(items, torch.int64, "items")
     return itemknn_scores(X, W, users, items.reshape(-1, 1)).reshape(-1)
+
+
+# ------------------------------------------------------------------ SLiM
+class SlimPanel:
+    """drb_slim_solve's result for targets begin .. begin + count - 1 (row r = item begin + r): the live coordinates lidx int32
+    [count, n] (ascending ids, the first nl[r] valid), their coefficients w fp64 and Z = q - G w fp64, and per target the
+    sweeps, the unscaled duality gap and whether it converged."""
+
+    def __init__(self, begin, lidx, w, z, nl, sweeps, gap, conv):
+        self.begin, self.lidx, self.w, self.z, self.nl = begin, lidx, w, z, nl
+        self.sweeps, self.gap, self.conv = sweeps, gap, conv
+
+    def dense(self):
+        """-> fp64 [count, n]: each target's full coefficient vector."""
+        count, n = self.lidx.shape
+        out = torch.zeros((count, n), dtype=torch.float64, device=self.w.device)
+        valid = torch.arange(n, device=self.w.device)[None, :] < self.nl[:, None].long()
+        rows = torch.arange(count, device=self.w.device)[:, None].expand(count, n)
+        out[rows[valid], self.lidx[valid].long()] = self.w[valid]
+        return out
+
+
+def slim_live(G, l1, begin=0, count=None, all_live=False):
+    """Items begin .. begin + count - 1 of G fp64 [n, n] = X^T X -> SlimPanel holding each item's live coordinates with w = 0 and
+    Z = q (sweeps / gap / conv not yet set).  all_live=False requires every stored value of X to be >= 0 (then coordinates with
+    G_kj <= l1, which never leave 0, are skipped exactly)."""
+    _dev(G, torch.float64, "G")
+    n = G.shape[0]
+    count = n - begin if count is None else count
+    dev = G.device
+    P = max(count, 1)
+    diag = torch.empty(n, dtype=torch.float64, device=dev)
+    lidx = torch.empty((P, n), dtype=torch.int32, device=dev)
+    w = torch.empty((P, n), dtype=torch.float64, device=dev)
+    z = torch.empty((P, n), dtype=torch.float64, device=dev)
+    nl = torch.empty(P, dtype=torch.int32, device=dev)
+    L.check(L.lib().drb_slim_live(_ptr(G), n, begin, count, float(l1), int(bool(all_live)), _ptr(diag), _ptr(lidx), _ptr(w), _ptr(z),
+                                  _ptr(nl), _stream()))
+    out = SlimPanel(begin, lidx[:count], w[:count], z[:count], nl[:count], None, None, None)
+    out.diag = diag
+    return out
+
+
+def slim_solve(G, l1, l2, tol, max_iter, begin=0, count=None, all_live=False, panel=None):
+    """SLiMRecommender.py:73-84 for items begin .. begin + count - 1 in Gram form on G fp64 [n, n] = X^T X -> SlimPanel.
+    ``panel``: slim_live's result for the same items (built here when None)."""
+    P = slim_live(G, l1, begin, count, all_live) if panel is None else panel
+    count, n = P.lidx.shape
+    dev = G.device
+    P.sweeps = torch.empty(max(count, 1), dtype=torch.int32, device=dev)[:count]
+    P.gap = torch.empty(max(count, 1), dtype=torch.float64, device=dev)[:count]
+    P.conv = torch.empty(max(count, 1), dtype=torch.int32, device=dev)[:count]
+    L.check(L.lib().drb_slim_solve(_ptr(G), n, P.begin, count, float(l1), float(l2), float(tol), int(max_iter), _ptr(P.diag),
+                                   _ptr(P.lidx), _ptr(P.w), _ptr(P.z), _ptr(P.nl), _ptr(P.sweeps), _ptr(P.gap), _ptr(P.conv),
+                                   _stream()))
+    return P
+
+
+def slim_select(panel, topk, out=None):
+    """:86-107 for a solved panel -> KnnNeighbours [n, topk] (rows of the panel's items written; pass ``out`` to fill one
+    KnnNeighbours panel by panel).  Per item the min(nnz - 1, topk) largest coefficients by (value desc, id asc), fp32."""
+    count, n = panel.lidx.shape
+    dev = panel.w.device
+    if out is None:
+        out = KnnNeighbours(torch.full((n, topk), -1, dtype=torch.int32, device=dev), torch.zeros((n, topk), dtype=torch.float32, device=dev),
+                            torch.zeros(n, dtype=torch.int32, device=dev))
+    L.check(L.lib().drb_slim_select(_ptr(panel.lidx), _ptr(panel.w), _ptr(panel.nl), n, panel.begin, count, topk, _ptr(out.idx),
+                                    _ptr(out.val), _ptr(out.cnt), _stream()))
+    return out

@@ -579,6 +579,32 @@ int drb_itemknn_scores(const int64_t *d_row_ptr, const int32_t *d_col, const flo
 int drb_itemknn_topk(const double *d_scores, int64_t n_rows, int32_t cand_num, const int64_t *d_cands, int32_t topk,
                      int64_t *d_out, void *stream);
 
+/* ---- SLiM: daisy/model/SLiMRecommender.py, csrc/slim.cu --------------------------------------------------------------------
+ * Item j's ElasticNet fit (:73-84) in Gram form on G = X^T X fp64 [n, n] (drb_ease_gram, reg 0), l1 = alpha elastic U,
+ * l2 = alpha (1 - elastic) U:  min_{w >= 0, w_j = 0} 1/2 w^T G w - G[:, j]^T w + l1 sum(w) + 1/2 l2 |w|^2.
+ * drb_slim_workspace_bytes  bytes of diag fp64 [n] and, for a panel of `panel` targets, d_lidx int32 / d_w fp64 / d_z fp64
+ *                           [panel, n] and d_nl int32 [panel].
+ * drb_slim_live             targets begin .. begin + count - 1, row r = target begin + r: d_diag = diag(G); d_lidx[r, :d_nl[r]]
+ *                           the live coordinates by ascending id (q_k > l1 when all_live == 0, which needs every stored value
+ *                           >= 0; else every k != j with G_kk > 0), d_w[r, :] = 0 and d_z[r, t] = q of item d_lidx[r, t].
+ * drb_slim_solve            on drb_slim_live's arrays: cyclic coordinate descent with sklearn's gap checks and stop at the
+ *                           formulation-A gap <= tol G_jj, at most max_iter sweeps; d_w[r, t] ends as the coefficient of item
+ *                           d_lidx[r, t], d_z as the matching q - G w.  Out per target: d_sweeps (sklearn's n_iter_), d_gap
+ *                           (unscaled: dual_gap_ * U), d_conv (1: converged, 0: stopped at max_iter).  Bitwise reproducible,
+ *                           and the same W for all_live 0 and 1.
+ * drb_slim_select           :86-107 for the solved panel: per target the min(nnz - 1, topk) largest coefficients by (value
+ *                           desc, id asc), fp32, by ascending id into rows begin .. of d_nbr_idx int32 [n, topk] (-1 past
+ *                           the count), d_nbr_val fp32 [n, topk], d_nbr_cnt int32 [n]: drb_itemknn_scores's layout.  topk in
+ *                           [1, 1024]. */
+size_t drb_slim_workspace_bytes(int32_t item_num, int32_t panel);
+int drb_slim_live(const double *d_G, int32_t item_num, int32_t begin, int32_t count, double l1, int32_t all_live, double *d_diag,
+                  int32_t *d_lidx, double *d_w, double *d_z, int32_t *d_nl, void *stream);
+int drb_slim_solve(const double *d_G, int32_t item_num, int32_t begin, int32_t count, double l1, double l2, double tol,
+                   int32_t max_iter, const double *d_diag, const int32_t *d_lidx, double *d_w, double *d_z, const int32_t *d_nl,
+                   int32_t *d_sweeps, double *d_gap, int32_t *d_conv, void *stream);
+int drb_slim_select(const int32_t *d_lidx, const double *d_w, const int32_t *d_nl, int32_t item_num, int32_t begin, int32_t count,
+                    int32_t topk, int32_t *d_nbr_idx, float *d_nbr_val, int32_t *d_nbr_cnt, void *stream);
+
 /* ---- evaluation: calc_ranking_results / Metric.run ------------------------------------------------
  * daisy/utils/metrics.py:18-57 (cut-off loop), :59-96 (dispatch), :98-251 (the KPIs).
  * d_preds: rank()'s float32 [n_users, ld] output; ground truth as CSR aligned with its rows
