@@ -13,6 +13,7 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 LIBDIR = os.path.join(HERE, "lib")
 SO = os.path.join(LIBDIR, "libdaisyrec_b200.so")
+HEADER = os.path.join(os.path.dirname(HERE), "include", "daisyrec_b200.h")
 SOURCES = ["capi.cu", "mf_bpr.cu", "sampler.cu", "rank.cu", "shard.cu", "lightgcn.cu", "neumf.cu", "comm.cu", "metrics.cu", "csr.cu", "randperm.cu", "p2p.cu", "ngcf.cu", "nfm.cu",
            "skipgram.cu", "item2vec.cu", "ease.cu", "itemknn.cu", "slim.cu"]
 ARCH = ["-gencode", "arch=compute_90a,code=sm_90a"]
@@ -36,7 +37,7 @@ def _stale(target, deps):
 def build(force=False, verbose=False):
     os.makedirs(LIBDIR, exist_ok=True)
     headers = [os.path.join(CSRC, f) for f in os.listdir(CSRC) if f.endswith((".cuh", ".h"))]
-    headers.append(os.path.join(os.path.dirname(HERE), "include", "daisyrec_b200.h"))
+    headers.append(HEADER)
     objs, procs = [], []
     for src in SOURCES:
         s = os.path.join(CSRC, src)

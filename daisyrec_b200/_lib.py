@@ -1,26 +1,17 @@
 """ctypes loader for libdaisyrec_b200.so -- the C ABI declared in include/daisyrec_b200.h.
 
+The header is the one declaration of that ABI: the restype / argtypes of every drb_* entry point and the DRB_* constants
+below are read from it, so a binding cannot drift from the prototype the compiler checks the definition against.
 The product path has NO CPU fallback: if the shared object is missing (and cannot be built
 because nvcc is absent) or a call fails, a RuntimeError is raised.
 """
 import ctypes as C
 import os
+import re
 
 from . import _build
 
 _lib = None
-
-c_i32p = C.POINTER(C.c_int32)
-c_i64p = C.POINTER(C.c_int64)
-c_u32p = C.POINTER(C.c_uint32)
-c_f32p = C.POINTER(C.c_float)
-c_f64p = C.POINTER(C.c_double)
-vp = C.c_void_p
-
-DRB_OK, DRB_ERR_INVALID, DRB_ERR_CUDA, DRB_ERR_NAN_LOSS, DRB_ERR_EMPTY_SET, DRB_ERR_NO_DEVICE, DRB_ERR_PEER, DRB_ERR_NOT_PD = range(8)
-OPT_SGD, OPT_ADAM, OPT_ADAGRAD, OPT_RMSPROP = 0, 1, 2, 3
-OPT_KIND = {"sgd": 0, "adam": 1, "adagrad": 2, "rmsprop": 3}
-LOSS_KIND = {"BPR": 0, "HL": 1, "TL": 2, "CL": 3, "SL": 4}
 
 
 class Hyper(C.Structure):
@@ -29,166 +20,70 @@ class Hyper(C.Structure):
                 ("beta1", C.c_float), ("beta2", C.c_float), ("eps", C.c_float), ("loss", C.c_int32)]
 
 
-# name -> (restype, argtypes); every symbol of include/daisyrec_b200.h
-SIGNATURES = {
-    "drb_version": (C.c_int, []),
-    "drb_last_error": (C.c_char_p, []),
-    "drb_device_query": (C.c_int, [c_i32p, c_i32p, c_i32p, c_i64p]),
-    "drb_index_range_check": (C.c_int, [vp, C.c_int32, C.c_int64, C.c_int32, c_i64p, c_i64p, vp]),
-    "drb_mf_step_variant": (C.c_int, [C.c_int32, C.c_int64, C.POINTER(C.c_int32), C.POINTER(C.c_int32)]),
-    "drb_mf_step_selfcheck_ms": (C.c_int, [C.c_int32, C.c_int64, C.POINTER(C.c_float), C.POINTER(C.c_float), C.POINTER(C.c_int32)]),
-    "drb_mf_last_step_mode": (C.c_int, []),
-    "drb_mf_step_geometry": (C.c_int, [C.c_int32, C.c_int32, C.POINTER(C.c_int32), C.POINTER(C.c_int32), C.c_int64,
-                                       C.POINTER(C.c_int32)]),
-    "drb_mt19937_seed": (C.c_int, [vp, C.c_uint32]),
-    "drb_sampler_draw_mt19937": (C.c_int, [vp, vp, C.c_int32, C.c_int32, C.c_int32, vp, c_i32p]),
-    "drb_sampler_draw_philox": (C.c_int, [C.c_uint64, C.c_uint64, vp, C.c_int32, C.c_int32, C.c_int32, vp, vp, vp]),
-    "drb_sampler_kth_complement": (C.c_int, [vp, vp, vp, C.c_int32, C.c_int32, C.c_int32, vp, vp]),
-    "drb_sampler_explode": (C.c_int, [vp, vp, C.c_int64, vp, C.c_int32, vp, vp]),
-    "drb_sample_triples_host": (C.c_int, [vp, vp, vp, vp, vp, C.c_int64, C.c_int32, C.c_int32, C.c_int32, vp, vp,
-                                          c_i32p]),
-    "drb_bounded_draws_mt19937": (C.c_int, [vp, vp, vp, C.c_int64, vp, c_i64p]),
-    "drb_kth_complement_var": (C.c_int, [vp, vp, vp, vp, C.c_int64, vp, vp]),
-    "drb_gather_triples": (C.c_int, [vp, vp, C.c_int64, vp, vp, vp, vp]),
-    "drb_mf_workspace_bytes": (C.c_size_t, [C.c_int32, C.c_int32, C.c_int32, C.c_int32]),
-    "drb_mf_workspace_init": (C.c_int, [vp, C.c_int32, C.c_int32, C.c_int32, C.c_int32, vp]),
-    "drb_mf_bpr_train_steps": (C.c_int, [vp, vp, vp, C.c_int32, C.c_int32, C.c_int32, vp, vp, vp, C.c_int64, C.c_int64,
-                                         C.c_int64, C.c_int64, C.POINTER(Hyper), C.c_int64, vp, C.c_int32, c_i64p, vp]),
-    "drb_mf_workspace_bytes_det": (C.c_size_t, [C.c_int32, C.c_int32, C.c_int32, C.c_int32]),
-    "drb_mf_bpr_train_steps_det": (C.c_int, [vp, vp, vp, C.c_int32, C.c_int32, C.c_int32, vp, vp, vp, C.c_int64, C.c_int64,
-                                             C.c_int64, C.c_int64, C.POINTER(Hyper), C.c_int64, vp, C.c_int32, c_i64p, vp]),
-    "drb_mf_bpr_train_steps_fused_neg": (C.c_int, [vp, vp, vp, C.c_int32, C.c_int32, C.c_int32, vp, vp, vp, vp, C.c_uint64, vp,
-                                                   C.c_int64, C.c_int64, C.c_int64, C.c_int64, C.POINTER(Hyper), C.c_int64, vp,
-                                                   C.c_int32, c_i64p, vp]),
-    "drb_mf_bpr_loss": (C.c_int, [vp, vp, vp, C.c_int32, C.c_int32, C.c_int32, vp, vp, vp, C.c_int64, C.POINTER(Hyper),
-                                  vp, vp]),
-    "drb_mf_bpr_train_step_host": (C.c_int, [vp, vp, vp, C.c_int32, C.c_int32, C.c_int32, vp, vp, vp, C.c_int64,
-                                             C.POINTER(Hyper), C.c_int64, vp, c_f64p, vp]),
-    "drb_mf_bpr_train_steps_host": (C.c_int, [vp, vp, vp, C.c_int32, C.c_int32, C.c_int32, vp, vp, vp, C.c_int64,
-                                              C.c_int64, C.c_int64, C.POINTER(Hyper), C.c_int64, vp, vp, vp, c_i64p, vp]),
-    "drb_randperm_workspace_bytes": (C.c_size_t, [C.c_int64]),
-    "drb_mt19937_stream": (C.c_int, [C.c_uint64, C.c_int64, vp, vp]),
-    "drb_mt19937_stream_variant": (C.c_int, [C.c_int64]),
-    "drb_randperm_torch": (C.c_int, [C.c_uint64, C.c_int64, vp, vp, vp]),
-    "drb_fm_workspace_bytes": (C.c_size_t, [C.c_int32, C.c_int32, C.c_int32, C.c_int32]),
-    "drb_fm_workspace_init": (C.c_int, [vp, C.c_int32, C.c_int32, C.c_int32, C.c_int32, vp]),
-    "drb_fm_train_steps": (C.c_int, [vp, vp, vp, vp, C.c_int32, C.c_int32, C.c_int32, vp, vp, vp, C.c_int64, C.c_int64,
-                                     C.c_int64, C.c_int64, C.POINTER(Hyper), C.c_int64, C.c_int32, vp, C.c_int32, c_i64p, vp]),
-    "drb_fm_rank": (C.c_int, [vp, vp, vp, C.c_int32, C.c_int32, C.c_int32, vp, C.c_int64, vp, C.c_int32, C.c_int32, vp, vp]),
-    "drb_fm_full_rank": (C.c_int, [vp, vp, vp, C.c_int32, C.c_int32, C.c_int32, vp, C.c_int64, C.c_int32, vp, vp]),
-    "drb_fm_predict": (C.c_int, [vp, vp, vp, C.c_int32, C.c_int32, C.c_int32, vp, vp, C.c_int64, vp, vp]),
-    "drb_mf_workspace_layout": (C.c_int, [C.c_int32, C.c_int32, C.c_int32, C.c_int32, c_i64p]),
-    "drb_mf_bpr_phase": (C.c_int, [vp, vp, vp, C.c_int32, C.c_int32, C.c_int32, vp, vp, vp, C.c_int64, C.c_int64,
-                                   C.c_int32, C.POINTER(Hyper), C.c_int64, vp, vp]),
-    "drb_shard_gather_triples": (C.c_int, [vp, vp, C.c_int64, C.c_int32, C.c_int32, C.c_int64, vp, vp, vp, vp, vp, vp]),
-    "drb_lgcn_segment_count": (C.c_int64, [vp, C.c_int64]),
-    "drb_lgcn_segments": (C.c_int, [vp, C.c_int64, vp, vp]),
-    "drb_lgcn_workspace_bytes": (C.c_size_t, [C.c_int32, C.c_int32, C.c_int32, C.c_int32]),
-    "drb_lgcn_workspace_init": (C.c_int, [vp, C.c_int32, C.c_int32, C.c_int32, C.c_int32, vp]),
-    "drb_lgcn_propagate": (C.c_int, [vp, vp, C.c_int32, C.c_int32, C.c_int32, C.c_int32, vp, vp, vp, vp, vp, C.c_int64, vp,
-                                     vp]),
-    "drb_lgcn_bpr_train_steps": (C.c_int, [vp, vp, C.c_int32, C.c_int32, C.c_int32, C.c_int32, vp, vp, vp, vp, vp,
-                                           C.c_int64, vp, vp, vp, C.c_int64, C.c_int64, C.c_int64, C.c_int64,
-                                           C.POINTER(Hyper), C.c_int64, C.c_int32, vp, C.c_int32, c_i64p, vp]),
-    "drb_ngcf_param_count": (C.c_int64, [c_i32p, C.c_int32]),
-    "drb_ngcf_workspace_bytes": (C.c_size_t, [C.c_int32, C.c_int32, c_i32p, C.c_int32, C.c_int32]),
-    "drb_ngcf_workspace_init": (C.c_int, [vp, C.c_int32, C.c_int32, c_i32p, C.c_int32, C.c_int32, vp]),
-    "drb_ngcf_forward": (C.c_int, [vp, vp, vp, C.c_int32, C.c_int32, c_i32p, C.c_int32, vp, vp, vp, vp, vp, C.c_int64, C.c_int32,
-                                   vp, vp]),
-    "drb_ngcf_bpr_train_steps": (C.c_int, [vp, vp, vp, C.c_int32, C.c_int32, c_i32p, C.c_int32, vp, vp, vp, vp, vp, C.c_int64,
-                                           vp, vp, vp, C.c_int64, C.c_int64, C.c_int64, C.c_int64, C.POINTER(Hyper), C.c_int64,
-                                           C.c_int32, C.c_int32, vp, C.c_int32, c_i64p, vp]),
-    "drb_ngcf_forward_dropout": (C.c_int, [vp, vp, vp, C.c_int32, C.c_int32, c_i32p, C.c_int32, vp, vp, vp, vp, vp, C.c_int64,
-                                           C.c_int32, vp, C.c_float, vp, vp]),
-    "drb_ngcf_bpr_train_steps_dropout": (C.c_int, [vp, vp, vp, C.c_int32, C.c_int32, c_i32p, C.c_int32, vp, vp, vp, vp, vp, C.c_int64,
-                                                   vp, vp, vp, C.c_int64, C.c_int64, C.c_int64, C.c_int64, C.POINTER(Hyper),
-                                                   C.c_int64, C.c_int32, C.c_int32, vp, C.c_float, vp, C.c_int32, c_i64p, vp]),
-    "drb_nfm_param_count": (C.c_int64, [C.c_int32, C.c_int32, C.c_int32]),
-    "drb_nfm_workspace_bytes": (C.c_size_t, [C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_int64]),
-    "drb_nfm_workspace_init": (C.c_int, [vp, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_int64, vp]),
-    "drb_nfm_bpr_train_steps": (C.c_int, [vp, vp, vp, vp, vp, vp, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_int32,
-                                          C.c_int32, C.c_int64, vp, vp, vp, C.c_int64, C.c_int64, C.c_int64, C.c_int64,
-                                          C.POINTER(Hyper), C.c_int64, C.c_int32, C.c_int32, vp, C.c_int32, c_i64p, vp]),
-    "drb_nfm_bpr_train_steps_dropout": (C.c_int, [vp, vp, vp, vp, vp, vp, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_int32,
-                                                  C.c_int32, C.c_int64, vp, vp, vp, C.c_int64, C.c_int64, C.c_int64, C.c_int64,
-                                                  C.POINTER(Hyper), C.c_int64, C.c_int32, C.c_int32, vp, C.c_float, vp, C.c_int32,
-                                                  c_i64p, vp]),
-    "drb_nfm_scores": (C.c_int, [vp, vp, vp, vp, vp, vp, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_int32,
-                                 C.c_int32, C.c_int64, vp, vp, C.c_int64, C.c_int32, vp, vp]),
-    "drb_comm_unique_id": (C.c_int, [vp]),
-    "drb_comm_init": (C.c_int, [vp, C.c_int32, C.c_int32]),
-    "drb_comm_destroy": (C.c_int, []),
-    "drb_mf_bpr_train_steps_sharded": (C.c_int, [vp, vp, vp, C.c_int32, C.c_int32, C.c_int32, vp, vp, vp, vp, C.c_int64,
-                                                 C.c_int64, C.POINTER(Hyper), C.c_int64, vp, vp]),
-    "drb_mf_bpr_train_steps_sharded_host": (C.c_int, [vp, vp, vp, C.c_int32, C.c_int32, C.c_int32, vp, vp, vp, vp,
-                                                      C.c_int64, C.c_int64, C.POINTER(Hyper), C.c_int64, vp, C.c_int64, vp,
-                                                      vp, vp]),
-    "drb_p2p_buffer_bytes": (C.c_size_t, [C.c_int32, C.c_int32]),
-    "drb_p2p_q_offset": (C.c_size_t, [C.c_int32, C.c_int32]),
-    "drb_p2p_alloc": (C.c_int, [C.c_size_t, C.POINTER(vp), vp]),
-    "drb_p2p_open": (C.c_int, [vp, C.POINTER(vp)]),
-    "drb_p2p_close": (C.c_int, [vp]),
-    "drb_p2p_free": (C.c_int, [vp]),
-    "drb_mf_bpr_train_steps_p2p": (C.c_int, [vp, vp, C.c_int32, C.c_int32, C.c_int32, C.POINTER(vp), C.c_int32, C.c_int32,
-                                             vp, vp, vp, vp, C.c_int64, C.c_int64, C.c_int64, C.c_int64, C.POINTER(Hyper),
-                                             C.c_int64, vp, C.c_double, C.c_int32, c_i64p, vp]),
-    "drb_neumf_param_count": (C.c_int64, [C.c_int32, C.c_int32, C.c_int32]),
-    "drb_neumf_mask_words": (C.c_int64, [C.c_int32, C.c_int32, C.c_int64]),
-    "drb_neumf_workspace_bytes": (C.c_size_t, [C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_int64]),
-    "drb_neumf_workspace_init": (C.c_int, [vp, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_int64, vp]),
-    "drb_neumf_bpr_train_steps": (C.c_int, [vp, vp, vp, vp, vp, vp, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_int64,
-                                            vp, vp, vp, C.c_int64, C.c_int64, C.c_int64, C.c_int64, C.POINTER(Hyper),
-                                            C.c_int64, C.c_int32, C.c_int32, C.c_float, C.c_uint64, vp, C.c_int32, vp,
-                                            C.c_int32, c_i64p, vp]),
-    "drb_neumf_scores": (C.c_int, [vp, vp, vp, vp, vp, vp, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_int64,
-                                   vp, C.c_int64, vp, C.c_int32, C.c_int32, C.c_int32, vp, vp]),
-    "drb_gemm_test": (C.c_int, [C.c_int32, C.c_int32, C.c_int64, C.c_int32, C.c_int32, vp, C.c_int64, vp, C.c_int64, vp,
-                                C.c_int64, vp, vp, C.c_int64, vp]),
-    "drb_topk_from_scores": (C.c_int, [vp, vp, C.c_int64, C.c_int32, C.c_int32, vp, vp, vp]),
-    "drb_mf_rank": (C.c_int, [vp, vp, C.c_int32, vp, C.c_int64, vp, C.c_int32, C.c_int32, vp, vp]),
-    "drb_mf_full_rank": (C.c_int, [vp, vp, C.c_int32, C.c_int32, vp, C.c_int64, C.c_int32, vp, vp]),
-    "drb_mf_predict": (C.c_int, [vp, vp, C.c_int32, vp, vp, C.c_int64, vp, vp]),
-    "drb_mf_rank_host": (C.c_int, [vp, vp, C.c_int32, vp, C.c_int64, vp, C.c_int32, C.c_int32, vp]),
-    "drb_sampler_draw_mt19937_mixed": (C.c_int, [vp, vp, C.c_int32, C.c_int32, C.c_int32, C.c_int32, vp, vp, c_i32p]),
-    "drb_sampler_assemble_mixed": (C.c_int, [vp, vp, vp, vp, vp, C.c_int32, C.c_int32, C.c_int32, C.c_int32, vp, vp]),
-    "drb_sampler_explode_pointwise": (C.c_int, [vp, vp, vp, C.c_int64, vp, C.c_int32, vp, vp]),
-    "drb_skipgram_workspace_bytes": (C.c_size_t, [C.c_int32, C.c_int64]),
-    "drb_skipgram_group": (C.c_int, [vp, C.c_int64, C.c_int32, C.c_int32, vp, vp, vp, vp, vp]),
-    "drb_skipgram_draws_mt19937": (C.c_int, [vp, vp, vp, C.c_int32, C.c_int32, vp, c_i32p]),
-    "drb_skipgram_emit": (C.c_int, [vp, vp, vp, C.c_int64, C.c_int32, vp, vp, vp, vp, vp, vp, vp]),
-    "drb_i2v_workspace_bytes": (C.c_size_t, [C.c_int32, C.c_int32, C.c_int32]),
-    "drb_i2v_workspace_init": (C.c_int, [vp, C.c_int32, C.c_int32, C.c_int32, vp]),
-    "drb_i2v_train_steps": (C.c_int, [vp, vp, C.c_int32, C.c_int32, vp, vp, vp, C.c_int64, C.c_int64, C.c_int64, C.c_int64,
-                                      C.POINTER(Hyper), C.c_int64, C.c_int32, vp, C.c_int32, c_i64p, vp]),
-    "drb_i2v_user_embedding": (C.c_int, [vp, C.c_int32, vp, vp, C.c_int32, vp, vp]),
-    "drb_csr_workspace_bytes": (C.c_size_t, [C.c_int32, C.c_int64]),
-    "drb_csr_build": (C.c_int, [vp, vp, C.c_int64, C.c_int32, C.c_int32, vp, vp, vp, c_i64p, vp]),
-    "drb_lgcn_build_adj": (C.c_int, [vp, vp, vp, vp, C.c_int32, C.c_int32, C.c_int64, vp, vp, vp, vp]),
-    "drb_ease_csr_workspace_bytes": (C.c_size_t, [C.c_int32, C.c_int64]),
-    "drb_ease_csr": (C.c_int, [vp, vp, vp, vp, C.c_int32, C.c_int32, vp, vp, C.c_int64, vp, vp, c_i32p, vp]),
-    "drb_ease_workspace_bytes": (C.c_size_t, [C.c_int32, C.c_int32, C.c_int32]),
-    "drb_ease_gram": (C.c_int, [vp, vp, vp, C.c_int32, C.c_int32, C.c_int32, C.c_double, vp, vp, vp]),
-    "drb_ease_inverse": (C.c_int, [vp, C.c_int32, vp, vp]),
-    "drb_ease_weights": (C.c_int, [vp, C.c_int32, vp, vp]),
-    "drb_ease_rank": (C.c_int, [vp, C.c_int32, vp, vp, vp, vp, C.c_int64, vp, C.c_int32, C.c_int32, vp, vp, vp]),
-    "drb_ease_full_rank": (C.c_int, [vp, C.c_int32, vp, vp, vp, vp, C.c_int32, C.c_int32, vp, vp, vp]),
-    "drb_ease_predict": (C.c_int, [vp, C.c_int32, vp, vp, vp, vp, vp, C.c_int64, vp, vp]),
-    "drb_ease_scale": (C.c_int, [vp, vp, vp, C.c_int32, C.c_int32, vp, c_i32p, vp]),
-    "drb_itemknn_transform": (C.c_int, [vp, vp, C.c_int32, C.c_int32, vp, vp, C.c_int32, C.c_int32, vp, vp, vp]),
-    "drb_itemknn_neighbours": (C.c_int, [vp, C.c_int32, vp, C.c_int32, C.c_int32, C.c_float, C.c_int32, vp, vp, vp, vp]),
-    "drb_itemknn_scores": (C.c_int, [vp, vp, vp, vp, vp, vp, C.c_int32, C.c_int32, vp, C.c_int64, vp, C.c_int32, vp, vp]),
-    "drb_itemknn_topk": (C.c_int, [vp, C.c_int64, C.c_int32, vp, C.c_int32, vp, vp]),
-    "drb_slim_workspace_bytes": (C.c_size_t, [C.c_int32, C.c_int32]),
-    "drb_slim_live": (C.c_int, [vp, C.c_int32, C.c_int32, C.c_int32, C.c_double, C.c_int32, vp, vp, vp, vp, vp, vp]),
-    "drb_slim_solve": (C.c_int, [vp, C.c_int32, C.c_int32, C.c_int32, C.c_double, C.c_double, C.c_double, C.c_int32,
-                                 vp, vp, vp, vp, vp, vp, vp, vp, vp]),
-    "drb_slim_select": (C.c_int, [vp, vp, vp, C.c_int32, C.c_int32, C.c_int32, C.c_int32, vp, vp, vp, vp]),
-    "drb_rank_metrics_workspace_bytes": (C.c_size_t, [C.c_int32, C.c_int32]),
-    "drb_rank_metrics": (C.c_int, [vp, C.c_int64, C.c_int32, vp, vp, vp, C.c_int32, C.c_int32, vp, vp, vp, vp]),
-    "drb_rank_metrics_host": (C.c_int, [vp, C.c_int64, C.c_int32, vp, vp, vp, C.c_int32, C.c_int32, vp, vp]),
-}
+def _header():
+    with open(_build.HEADER) as f:
+        return f.read()
 
-KPI_NAMES = ("recall", "mrr", "ndcg", "hit", "precision", "map", "coverage", "popularity")   # DRB_KPI_* order
+
+def defines(text):
+    """name -> value of every `#define DRB_* <integer>` of the C text."""
+    return {m[1]: int(m[2]) for m in re.finditer(r"^\s*#define\s+(DRB_\w+)\s+(-?\d+)\b", text, re.M)}
+
+
+def prototypes(text):
+    """name -> (return type, [parameter types]) of every drb_* prototype of the C text, the types as C spells them."""
+    text = re.sub(r"/\*.*?\*/|//[^\n]*", " ", text, flags=re.S)          # comments
+    text = re.sub(r"^\s*#[^\n]*", "", text, flags=re.M)                    # preprocessor lines
+    out = {}
+    for decl in re.split(r"[;{}]", text):
+        m = re.fullmatch(r"\s*(.*?)\b(drb_\w+)\s*\((.*)\)\s*", decl, re.S)
+        if m is None:
+            continue
+        ret, name, params = m.groups()
+        params = [p.strip() for p in params.split(",")]
+        params = [] if params == ["void"] else [re.sub(r"\w+$", "", p).strip() for p in params]     # drop the names
+        out[name] = (ret.strip(), params)
+    return out
+
+
+_SCALARS = {"int": C.c_int, "int32_t": C.c_int32, "int64_t": C.c_int64, "uint32_t": C.c_uint32, "uint64_t": C.c_uint64,
+            "uint8_t": C.c_uint8, "unsigned long long": C.c_ulonglong, "size_t": C.c_size_t, "float": C.c_float,
+            "double": C.c_double}
+
+
+def ctype(decl, fn, ret=False):
+    """ctypes type of the C type ``decl`` in the signature of ``fn`` (its return type when ``ret``): the scalars by value,
+    a returned `const char *` as c_char_p, `void **` as POINTER(c_void_p), `drb_hyper *` as POINTER(Hyper) and every other
+    pointer as c_void_p.  ValueError for a type outside these."""
+    stars = decl.count("*")
+    base = " ".join(w for w in re.findall(r"\w+", decl) if w != "const")
+    if stars == 0 and base in _SCALARS:
+        return _SCALARS[base]
+    if stars == 1 and base == "char" and ret:
+        return C.c_char_p
+    if stars == 2 and base == "void":
+        return C.POINTER(C.c_void_p)
+    if stars == 1 and base == "drb_hyper":
+        return C.POINTER(Hyper)
+    if stars and (base in _SCALARS or base in ("void", "char", "drb_hyper")):
+        return C.c_void_p
+    raise ValueError(f"{fn}: unknown C type '{decl}' in include/daisyrec_b200.h")
+
+
+def signatures(text):
+    """name -> (restype, argtypes) of every drb_* prototype of the C text."""
+    return {name: (ctype(ret, name, ret=True), [ctype(p, name) for p in params])
+            for name, (ret, params) in prototypes(text).items()}
+
+
+_DEFINES = defines(_header())
+DRB_OK = _DEFINES["DRB_OK"]
+globals().update((k, v) for k, v in _DEFINES.items() if k.startswith("DRB_ERR_"))     # DRB_ERR_INVALID, DRB_ERR_CUDA, ...
+OPT_KIND = {k.removeprefix("DRB_OPT_").lower(): v for k, v in _DEFINES.items() if k.startswith("DRB_OPT_")}
+OPT_SGD, OPT_ADAM = OPT_KIND["sgd"], OPT_KIND["adam"]
+LOSS_KIND = {k.removeprefix("DRB_LOSS_"): v for k, v in _DEFINES.items() if k.startswith("DRB_LOSS_")}
+KPI_NAMES = tuple(k.removeprefix("DRB_KPI_").lower() for k in sorted(_DEFINES, key=_DEFINES.get)
+                  if k.startswith("DRB_KPI_") and k != "DRB_KPI_COUNT")                 # DRB_KPI_* order
 
 
 def so_path():
@@ -260,7 +155,7 @@ def lib():
                 f"libdaisyrec_b200.so is missing ({path}) and could not be built: {e}. "
                 "The GPU path has no CPU fallback; run `python -c 'import __graft_entry__ as g; g.build()'`.") from e
     L = C.CDLL(path)
-    for name, (res, args) in SIGNATURES.items():
+    for name, (res, args) in signatures(_header()).items():
         fn = getattr(L, name)          # AttributeError here == header and library out of sync
         fn.restype, fn.argtypes = res, args
     _canary(path)
@@ -274,9 +169,11 @@ class DrbError(RuntimeError):
         self.code = code
 
 
-# the errors the reference raises for these conditions (AbstractRecommender.py:122-123; numpy's choice() on an empty population)
+# the errors the reference raises for these conditions (AbstractRecommender.py:122-123; numpy's choice() on an empty population;
+# BatchNorm1d given one row in training mode)
 NAN_LOSS_MESSAGE = "Loss=Nan or Infinity: current settings does not fit the recommender"
 EMPTY_SET_MESSAGE = "'a' cannot be empty unless no samples are taken"
+BATCHNORM_MESSAGE = "Expected more than 1 value per channel"
 
 
 def check(rc):
@@ -286,7 +183,10 @@ def check(rc):
         raise ValueError(NAN_LOSS_MESSAGE)
     if rc == DRB_ERR_EMPTY_SET:
         raise ValueError(EMPTY_SET_MESSAGE)
+    msg = (lib().drb_last_error() or b"").decode(errors="replace")
     if rc == DRB_ERR_NOT_PD:
         import numpy as np
-        raise np.linalg.LinAlgError((lib().drb_last_error() or b"").decode(errors="replace"))
-    raise DrbError(rc, (lib().drb_last_error() or b"").decode(errors="replace"))
+        raise np.linalg.LinAlgError(msg)
+    if rc == DRB_ERR_INVALID and msg.startswith(BATCHNORM_MESSAGE):
+        raise ValueError(msg)
+    raise DrbError(rc, msg)

@@ -510,30 +510,17 @@ extern "C" int drb_nfm_workspace_init(void *d_ws, int32_t U, int32_t I, int32_t 
 }
 
 // n_steps synchronous NFM + BPR steps (apply != 0) or the loss of one batch (apply == 0: like calc_loss under train(), the
-// BatchNorm running statistics still move).  act: 0 relu, 1 sigmoid, 2 tanh.
+// BatchNorm running statistics still move).  act: 0 relu, 1 sigmoid, 2 tanh.  nn.Dropout is active when d_keep != NULL
+// (dropout = config['dropout'] > 0, the reference default 0.5).  d_keep: the masks torch's Dropout modules draw, as bytes (0 / 1),
+// for the n_steps steps in order: per step [forward call: pos, neg][site: FM_layers' Dropout, then the one behind each
+// activation][batch][F] (the caller draws them on torch's CPU generator in exactly that order; a ragged last batch uses its own
+// row count).  Every step must hold `batch` triples when n_steps > 1.  d_keep = NULL: no dropout.
 extern "C" int drb_nfm_bpr_train_steps(float *d_P, float *d_Q, float *d_bias, float *d_N, float *d_Rs, void *d_ws, int32_t U,
                                        int32_t I, int32_t F, int32_t L, int32_t batch_norm, int32_t act, int64_t max_rows,
                                        const int32_t *d_bu, const int32_t *d_bi, const int32_t *d_bj, int64_t n, int64_t batch,
                                        int64_t first_step, int64_t n_steps, const drb_hyper *h, int64_t adam_step0, int32_t apply,
-                                       int32_t tower_dtype, double *d_step_loss, int32_t sync_and_check, int64_t *nan_step,
-                                       void *stream)
-{
-    return drb_nfm_bpr_train_steps_dropout(d_P, d_Q, d_bias, d_N, d_Rs, d_ws, U, I, F, L, batch_norm, act, max_rows, d_bu, d_bi, d_bj,
-                                           n, batch, first_step, n_steps, h, adam_step0, apply, tower_dtype, nullptr, 0.f,
-                                           d_step_loss, sync_and_check, nan_step, stream);
-}
-
-// The same with nn.Dropout active (dropout = config['dropout'] > 0, the reference default 0.5).  d_keep: the masks torch's Dropout
-// modules draw, as bytes (0 / 1), for the n_steps steps in order: per step [forward call: pos, neg][site: FM_layers' Dropout, then
-// the one behind each activation][batch][F] (the caller draws them on torch's CPU generator in exactly that order; a ragged
-// last batch uses its own row count).  Every step must hold `batch` triples when n_steps > 1.
-extern "C" int drb_nfm_bpr_train_steps_dropout(float *d_P, float *d_Q, float *d_bias, float *d_N, float *d_Rs, void *d_ws, int32_t U,
-                                               int32_t I, int32_t F, int32_t L, int32_t batch_norm, int32_t act, int64_t max_rows,
-                                               const int32_t *d_bu, const int32_t *d_bi, const int32_t *d_bj, int64_t n,
-                                               int64_t batch, int64_t first_step, int64_t n_steps, const drb_hyper *h,
-                                               int64_t adam_step0, int32_t apply, int32_t tower_dtype, const uint8_t *d_keep,
-                                               float dropout, double *d_step_loss, int32_t sync_and_check, int64_t *nan_step,
-                                               void *stream)
+                                       int32_t tower_dtype, const uint8_t *d_keep, float dropout, double *d_step_loss,
+                                       int32_t sync_and_check, int64_t *nan_step, void *stream)
 {
     NfmDims d;
     DRB_REQUIRE(d_keep == nullptr || (dropout > 0.f && dropout < 1.f), "nfm: dropout masks need 0 < dropout < 1");

@@ -340,22 +340,13 @@ extern "C" int drb_ngcf_workspace_init(void *d_ws, int32_t U, int32_t I, const i
     return DRB_OK;
 }
 
-// NGCF.forward: d_out [n, C] = cat(E_0 .. E_L, dim=1)
+// NGCF.forward: d_out [n, C] = cat(E_0 .. E_L, dim=1), with nn.Dropout(mess_dropout) of :164 active when d_keep != NULL (the
+// reference's module is always in training mode, rank() included).  d_keep: the masks torch draws, one per layer over its
+// [n, width] output, as bytes, layers concatenated; NULL = no dropout.
 extern "C" int drb_ngcf_forward(const float *d_E0, const float *d_W, void *d_ws, int32_t U, int32_t I, const int32_t *dims,
                                 int32_t L, const int64_t *d_row_ptr, const int32_t *d_col, const float *d_val,
                                 const int32_t *d_seg_row, const int64_t *d_seg_ptr, int64_t nseg, int32_t tower_dtype,
-                                float *d_out, void *stream)
-{
-    return drb_ngcf_forward_dropout(d_E0, d_W, d_ws, U, I, dims, L, d_row_ptr, d_col, d_val, d_seg_row, d_seg_ptr, nseg, tower_dtype,
-                                    nullptr, 0.f, d_out, stream);
-}
-
-// forward() with nn.Dropout(mess_dropout) active (:164; the reference's module is always in training mode, rank() included).
-// d_keep: the masks torch draws, one per layer over its [n, width] output, as bytes, layers concatenated; NULL = no dropout.
-extern "C" int drb_ngcf_forward_dropout(const float *d_E0, const float *d_W, void *d_ws, int32_t U, int32_t I, const int32_t *dims,
-                                        int32_t L, const int64_t *d_row_ptr, const int32_t *d_col, const float *d_val,
-                                        const int32_t *d_seg_row, const int64_t *d_seg_ptr, int64_t nseg, int32_t tower_dtype,
-                                        const uint8_t *d_keep, float dropout, float *d_out, void *stream)
+                                const uint8_t *d_keep, float dropout, float *d_out, void *stream)
 {
     NgcfDims q;
     DRB_REQUIRE(d_keep == nullptr || (dropout > 0.f && dropout < 1.f), "ngcf: dropout masks need 0 < mess_dropout < 1");
@@ -372,30 +363,16 @@ extern "C" int drb_ngcf_forward_dropout(const float *d_E0, const float *d_W, voi
     return DRB_OK;
 }
 
-// n_steps synchronous NGCF + BPR steps (apply != 0) or the loss of one batch (apply == 0).
+// n_steps synchronous NGCF + BPR steps (apply != 0) or the loss of one batch (apply == 0), with the message dropout of :164
+// active when d_keep != NULL (reference default mess_dropout 0.1).  d_keep: per step the masks of the one forward() a step runs
+// (layers concatenated, bytes), steps concatenated; NULL = no dropout.
 extern "C" int drb_ngcf_bpr_train_steps(float *d_E0, float *d_W, void *d_ws, int32_t U, int32_t I, const int32_t *dims, int32_t L,
                                         const int64_t *d_row_ptr, const int32_t *d_col, const float *d_val,
                                         const int32_t *d_seg_row, const int64_t *d_seg_ptr, int64_t nseg, const int32_t *d_bu,
                                         const int32_t *d_bi, const int32_t *d_bj, int64_t n_triples, int64_t batch,
                                         int64_t first_step, int64_t n_steps, const drb_hyper *h, int64_t adam_step0,
-                                        int32_t apply, int32_t tower_dtype, double *d_step_loss, int32_t sync_and_check,
-                                        int64_t *nan_step, void *stream)
-{
-    return drb_ngcf_bpr_train_steps_dropout(d_E0, d_W, d_ws, U, I, dims, L, d_row_ptr, d_col, d_val, d_seg_row, d_seg_ptr, nseg, d_bu,
-                                            d_bi, d_bj, n_triples, batch, first_step, n_steps, h, adam_step0, apply, tower_dtype,
-                                            nullptr, 0.f, d_step_loss, sync_and_check, nan_step, stream);
-}
-
-// The same with the message dropout of :164 active (reference default mess_dropout 0.1).  d_keep: per step the masks of the one
-// forward() a step runs (layers concatenated, bytes), steps concatenated.
-extern "C" int drb_ngcf_bpr_train_steps_dropout(float *d_E0, float *d_W, void *d_ws, int32_t U, int32_t I, const int32_t *dims,
-                                                int32_t L, const int64_t *d_row_ptr, const int32_t *d_col, const float *d_val,
-                                                const int32_t *d_seg_row, const int64_t *d_seg_ptr, int64_t nseg,
-                                                const int32_t *d_bu, const int32_t *d_bi, const int32_t *d_bj, int64_t n_triples,
-                                                int64_t batch, int64_t first_step, int64_t n_steps, const drb_hyper *h,
-                                                int64_t adam_step0, int32_t apply, int32_t tower_dtype, const uint8_t *d_keep,
-                                                float dropout, double *d_step_loss, int32_t sync_and_check, int64_t *nan_step,
-                                                void *stream)
+                                        int32_t apply, int32_t tower_dtype, const uint8_t *d_keep, float dropout,
+                                        double *d_step_loss, int32_t sync_and_check, int64_t *nan_step, void *stream)
 {
     NgcfDims q;
     DRB_REQUIRE(d_keep == nullptr || (dropout > 0.f && dropout < 1.f), "ngcf: dropout masks need 0 < mess_dropout < 1");

@@ -25,6 +25,15 @@ def _dev(t, dtype, name):
     return t
 
 
+def _train_steps(fn, n_steps, device, check, *args, out=None):
+    """Calls a step entry point with ``args`` followed by its trailing (d_step_loss, sync_and_check, nan_step, stream)
+    arguments -> float64 device losses [n_steps] (in ``out`` when given)."""
+    losses = out if out is not None else torch.empty(max(n_steps, 1), dtype=torch.float64, device=device)
+    nan_step = C.c_int64(-1)
+    L.check(fn(*args, _ptr(losses), 1 if check else 0, C.byref(nan_step), _stream()))
+    return losses[:n_steps]
+
+
 def require_cuda():
     if not torch.cuda.is_available():
         raise RuntimeError("daisyrec_b200 needs a CUDA device (sm_90a); there is no CPU fallback")
@@ -356,14 +365,9 @@ def mf_bpr_train_steps(P, Q, ws, bu, bi, bj, batch, first_step, n_steps, hp, ada
     _dev(P, torch.float32, "P"); _dev(Q, torch.float32, "Q")
     for t, nm in ((bu, "bu"), (bi, "bi"), (bj, "bj")):
         _dev(t, torch.int32, nm)
-    n = bu.numel()
-    losses = out if out is not None else torch.empty(max(n_steps, 1), dtype=torch.float64, device=P.device)
-    nan_step = C.c_int64(-1)
     fn = L.lib().drb_mf_bpr_train_steps_det if getattr(ws, "det", False) else L.lib().drb_mf_bpr_train_steps
-    rc = fn(_ptr(P), _ptr(Q), _ptr(ws.buf), ws.U, ws.I, ws.F, _ptr(bu), _ptr(bi), _ptr(bj), n, batch, first_step, n_steps,
-            C.byref(hp), adam_step0, _ptr(losses), 1 if check else 0, C.byref(nan_step), _stream())
-    L.check(rc)
-    return losses[:n_steps]
+    return _train_steps(fn, n_steps, P.device, check, _ptr(P), _ptr(Q), _ptr(ws.buf), ws.U, ws.I, ws.F, _ptr(bu), _ptr(bi),
+                        _ptr(bj), bu.numel(), batch, first_step, n_steps, C.byref(hp), adam_step0, out=out)
 
 
 def mf_bpr_train_steps_fused_neg(P, Q, ws, bu, bi, d_row_ptr, d_col, seed, batch, first_step, n_steps, hp, adam_step0=0,
@@ -372,15 +376,9 @@ def mf_bpr_train_steps_fused_neg(P, Q, ws, bu, bi, d_row_ptr, d_col, seed, batch
     user's CSR row.  neg_out (optional int32 [n]) receives them."""
     _dev(P, torch.float32, "P"); _dev(Q, torch.float32, "Q"); _dev(bu, torch.int32, "bu"); _dev(bi, torch.int32, "bi")
     _dev(d_row_ptr, torch.int64, "row_ptr"); _dev(d_col, torch.int32, "col")
-    losses = torch.empty(max(n_steps, 1), dtype=torch.float64, device=P.device)
-    nan_step = C.c_int64(-1)
-    rc = L.lib().drb_mf_bpr_train_steps_fused_neg(_ptr(P), _ptr(Q), _ptr(ws.buf), ws.U, ws.I, ws.F, _ptr(bu), _ptr(bi),
-                                                  _ptr(d_row_ptr), _ptr(d_col), C.c_uint64(seed),
-                                                  None if neg_out is None else _ptr(neg_out), bu.numel(), batch, first_step,
-                                                  n_steps, C.byref(hp), adam_step0, _ptr(losses), 1 if check else 0,
-                                                  C.byref(nan_step), _stream())
-    L.check(rc)
-    return losses[:n_steps]
+    return _train_steps(L.lib().drb_mf_bpr_train_steps_fused_neg, n_steps, P.device, check, _ptr(P), _ptr(Q), _ptr(ws.buf), ws.U,
+                        ws.I, ws.F, _ptr(bu), _ptr(bi), _ptr(d_row_ptr), _ptr(d_col), C.c_uint64(seed),
+                        None if neg_out is None else _ptr(neg_out), bu.numel(), batch, first_step, n_steps, C.byref(hp), adam_step0)
 
 
 def mf_bpr_loss(P, Q, ws, bu, bi, bj, hp):
@@ -442,12 +440,8 @@ def i2v_train_steps(Q, ws, bt, bc, blabel, batch, first_step, n_steps, hp, adam_
     _dev(Q, torch.float32, "Q")
     for t, nm in ((bt, "target"), (bc, "context"), (blabel, "label")):
         _dev(t, torch.int32, nm)
-    losses = torch.empty(max(n_steps, 1), dtype=torch.float64, device=Q.device)
-    nan_step = C.c_int64(-1)
-    L.check(L.lib().drb_i2v_train_steps(_ptr(Q), _ptr(ws.buf), ws.I, ws.F, _ptr(bt), _ptr(bc), _ptr(blabel), bt.numel(), batch,
-                                        first_step, n_steps, C.byref(hp), adam_step0, 1 if apply else 0, _ptr(losses),
-                                        1 if check else 0, C.byref(nan_step), _stream()))
-    return losses[:n_steps]
+    return _train_steps(L.lib().drb_i2v_train_steps, n_steps, Q.device, check, _ptr(Q), _ptr(ws.buf), ws.I, ws.F, _ptr(bt), _ptr(bc),
+                        _ptr(blabel), bt.numel(), batch, first_step, n_steps, C.byref(hp), adam_step0, 1 if apply else 0)
 
 
 def i2v_user_embedding(Q, d_row_ptr, d_col, P):
@@ -476,13 +470,9 @@ def fm_train_steps(P, Q, bias, ws, bu, bi, bj, batch, first_step, n_steps, hp, a
         _dev(t, torch.int32, nm)
     if bias.numel() != ws.U + ws.I + 1:
         raise ValueError("bias must hold user_num + item_num + 1 floats")
-    losses = torch.empty(max(n_steps, 1), dtype=torch.float64, device=P.device)
-    nan_step = C.c_int64(-1)
-    rc = L.lib().drb_fm_train_steps(_ptr(P), _ptr(Q), _ptr(bias), _ptr(ws.buf), ws.U, ws.I, ws.F, _ptr(bu), _ptr(bi), _ptr(bj),
-                                    bu.numel(), batch, first_step, n_steps, C.byref(hp), adam_step0, 1 if apply else 0,
-                                    _ptr(losses), 1 if check else 0, C.byref(nan_step), _stream())
-    L.check(rc)
-    return losses[:n_steps]
+    return _train_steps(L.lib().drb_fm_train_steps, n_steps, P.device, check, _ptr(P), _ptr(Q), _ptr(bias), _ptr(ws.buf), ws.U,
+                        ws.I, ws.F, _ptr(bu), _ptr(bi), _ptr(bj), bu.numel(), batch, first_step, n_steps, C.byref(hp), adam_step0,
+                        1 if apply else 0)
 
 
 def fm_rank(P, Q, bias, users, cands, topk):
@@ -611,14 +601,9 @@ def lgcn_bpr_train_steps(E0, ws, graph, num_layers, bu, bi, bj, batch, first_ste
     _dev(E0, torch.float32, "E0")
     for t, nm in ((bu, "bu"), (bi, "bi"), (bj, "bj")):
         _dev(t, torch.int32, nm)
-    losses = torch.empty(max(1, n_steps), dtype=torch.float64, device=E0.device)
-    nan_step = C.c_int64(-1)
-    rc = L.lib().drb_lgcn_bpr_train_steps(_ptr(E0), _ptr(ws.buf), ws.U, ws.I, ws.F, num_layers, *graph.args(), _ptr(bu),
-                                          _ptr(bi), _ptr(bj), bu.numel(), batch, first_step, n_steps, C.byref(hp),
-                                          adam_step0, 1 if apply else 0, _ptr(losses), 1 if check else 0,
-                                          C.byref(nan_step), _stream())
-    L.check(rc)
-    return losses[:n_steps]
+    return _train_steps(L.lib().drb_lgcn_bpr_train_steps, n_steps, E0.device, check, _ptr(E0), _ptr(ws.buf), ws.U, ws.I, ws.F,
+                        num_layers, *graph.args(), _ptr(bu), _ptr(bi), _ptr(bj), bu.numel(), batch, first_step, n_steps,
+                        C.byref(hp), adam_step0, 1 if apply else 0)
 
 
 # ------------------------------------------------------------------ NGCF
@@ -655,9 +640,9 @@ def ngcf_forward(E0, W, ws, graph, tower_dtype=0, dropout=0.0, keep=None):
         if keep.numel() != ngcf_keep_bytes(ws):
             raise ValueError("keep must hold (user_num + item_num) x sum(hidden widths) bytes")
     out = torch.empty((ws.U + ws.I, sum(ws.dims)), dtype=torch.float32, device=E0.device)
-    L.check(L.lib().drb_ngcf_forward_dropout(_ptr(E0), _ptr(W), _ptr(ws.buf), ws.U, ws.I, _dims_arr(ws.dims), len(ws.dims) - 1,
-                                             *graph.args(), tower_dtype, None if keep is None else _ptr(keep),
-                                             C.c_float(dropout if keep is not None else 0.0), _ptr(out), _stream()))
+    L.check(L.lib().drb_ngcf_forward(_ptr(E0), _ptr(W), _ptr(ws.buf), ws.U, ws.I, _dims_arr(ws.dims), len(ws.dims) - 1,
+                                     *graph.args(), tower_dtype, None if keep is None else _ptr(keep),
+                                     C.c_float(dropout if keep is not None else 0.0), _ptr(out), _stream()))
     return out
 
 
@@ -670,16 +655,10 @@ def ngcf_bpr_train_steps(E0, W, ws, graph, bu, bi, bj, batch, first_step, n_step
         _dev(keep, torch.uint8, "keep")
         if keep.numel() != max(1, n_steps) * ngcf_keep_bytes(ws):
             raise ValueError("keep must hold n_steps x (user_num + item_num) x sum(hidden widths) bytes")
-    losses = torch.empty(max(1, n_steps), dtype=torch.float64, device=E0.device)
-    nan_step = C.c_int64(-1)
-    rc = L.lib().drb_ngcf_bpr_train_steps_dropout(_ptr(E0), _ptr(W), _ptr(ws.buf), ws.U, ws.I, _dims_arr(ws.dims), len(ws.dims) - 1,
-                                                  *graph.args(), _ptr(bu), _ptr(bi), _ptr(bj), bu.numel(), batch, first_step,
-                                                  n_steps, C.byref(hp), adam_step0, 1 if apply else 0, tower_dtype,
-                                                  None if keep is None else _ptr(keep),
-                                                  C.c_float(dropout if keep is not None else 0.0), _ptr(losses),
-                                                  1 if check else 0, C.byref(nan_step), _stream())
-    L.check(rc)
-    return losses[:n_steps]
+    return _train_steps(L.lib().drb_ngcf_bpr_train_steps, n_steps, E0.device, check, _ptr(E0), _ptr(W), _ptr(ws.buf), ws.U, ws.I,
+                        _dims_arr(ws.dims), len(ws.dims) - 1, *graph.args(), _ptr(bu), _ptr(bi), _ptr(bj), bu.numel(), batch,
+                        first_step, n_steps, C.byref(hp), adam_step0, 1 if apply else 0, tower_dtype,
+                        None if keep is None else _ptr(keep), C.c_float(dropout if keep is not None else 0.0))
 
 
 # ------------------------------------------------------------------ NFM
@@ -705,7 +684,7 @@ class NfmWorkspace:
 def nfm_bpr_train_steps(P, Q, bias, N, Rs, ws, act, bu, bi, bj, batch, first_step, n_steps, hp, adam_step0=0, apply=True,
                         check=True, tower_dtype=0, dropout=0.0, keep=None):
     """keep (with dropout > 0): uint8 CUDA tensor of the masks torch's Dropout modules draw, per step
-    [forward call][site][batch][F] (drb_nfm_bpr_train_steps_dropout)."""
+    [forward call][site][batch][F] (drb_nfm_bpr_train_steps)."""
     for t in (P, Q, bias, N):
         _dev(t, torch.float32, "parameter")
     for t, nm in ((bu, "bu"), (bi, "bi"), (bj, "bj")):
@@ -715,19 +694,11 @@ def nfm_bpr_train_steps(P, Q, bias, N, Rs, ws, act, bu, bi, bj, batch, first_ste
         rows = batch if n_steps != 1 else min(batch, bu.numel() - first_step * batch)
         if keep.numel() != max(1, n_steps) * 2 * (1 + ws.Ln) * rows * ws.F:
             raise ValueError("keep must hold n_steps x 2 x (1 + num_layers) x batch x factors bytes")
-    losses = torch.empty(max(1, n_steps), dtype=torch.float64, device=P.device)
-    nan_step = C.c_int64(-1)
-    rc = L.lib().drb_nfm_bpr_train_steps_dropout(
-        _ptr(P), _ptr(Q), _ptr(bias), _ptr(N), None if Rs is None or Rs.numel() == 0 else _ptr(Rs), _ptr(ws.buf), ws.U, ws.I, ws.F,
-        ws.Ln, ws.bn, act, ws.max_rows, _ptr(bu), _ptr(bi), _ptr(bj), bu.numel(), batch, first_step, n_steps, C.byref(hp), adam_step0,
-        1 if apply else 0, tower_dtype, None if keep is None else _ptr(keep), C.c_float(dropout if keep is not None else 0.0),
-        _ptr(losses), 1 if check else 0, C.byref(nan_step), _stream())
-    if rc == L.DRB_ERR_INVALID:
-        msg = (L.lib().drb_last_error() or b"").decode(errors="replace")
-        if msg.startswith("Expected more than 1 value per channel"):      # BatchNorm1d's own ValueError in the reference
-            raise ValueError(msg)
-    L.check(rc)
-    return losses[:n_steps]
+    return _train_steps(
+        L.lib().drb_nfm_bpr_train_steps, n_steps, P.device, check, _ptr(P), _ptr(Q), _ptr(bias), _ptr(N),
+        None if Rs is None or Rs.numel() == 0 else _ptr(Rs), _ptr(ws.buf), ws.U, ws.I, ws.F, ws.Ln, ws.bn, act, ws.max_rows, _ptr(bu),
+        _ptr(bi), _ptr(bj), bu.numel(), batch, first_step, n_steps, C.byref(hp), adam_step0, 1 if apply else 0, tower_dtype,
+        None if keep is None else _ptr(keep), C.c_float(dropout if keep is not None else 0.0))
 
 
 def nfm_scores(P, Q, bias, N, Rs, ws, act, u, i, tower_dtype=0):
@@ -775,16 +746,10 @@ def neumf_bpr_train_steps(tabs, W, ws, bu, bi, bj, batch, first_step, n_steps, h
         _dev(t, torch.float32, "table")
     for t, nm in ((bu, "bu"), (bi, "bi"), (bj, "bj")):
         _dev(t, torch.int32, nm)
-    losses = torch.empty(max(1, n_steps), dtype=torch.float64, device=W.device)
-    nan_step = C.c_int64(-1)
-    rc = L.lib().drb_neumf_bpr_train_steps(_ptr(tabs[0]), _ptr(tabs[1]), _ptr(tabs[2]), _ptr(tabs[3]), _ptr(W), _ptr(ws.buf),
-                                           ws.U, ws.I, ws.F, ws.Ln, ws.max_rows, _ptr(bu), _ptr(bi), _ptr(bj), bu.numel(),
-                                           batch, first_step, n_steps, C.byref(hp), adam_step0, 1 if apply else 0,
-                                           tower_dtype, C.c_float(dropout), C.c_uint64(dropout_seed),
-                                           None if drop_masks is None else _ptr(drop_masks), mode, _ptr(losses),
-                                           1 if check else 0, C.byref(nan_step), _stream())
-    L.check(rc)
-    return losses[:n_steps]
+    return _train_steps(L.lib().drb_neumf_bpr_train_steps, n_steps, W.device, check, _ptr(tabs[0]), _ptr(tabs[1]), _ptr(tabs[2]),
+                        _ptr(tabs[3]), _ptr(W), _ptr(ws.buf), ws.U, ws.I, ws.F, ws.Ln, ws.max_rows, _ptr(bu), _ptr(bi), _ptr(bj),
+                        bu.numel(), batch, first_step, n_steps, C.byref(hp), adam_step0, 1 if apply else 0, tower_dtype,
+                        C.c_float(dropout), C.c_uint64(dropout_seed), None if drop_masks is None else _ptr(drop_masks), mode)
 
 
 def neumf_scores(tabs, W, ws, users, items, per_user, tower_dtype=0, mode=0):

@@ -13,16 +13,76 @@ import torch
 from conftest import ROOT, golden, csr_from_coo
 
 
-def test_library_exports_every_header_symbol():
+def _header():
+    return open(os.path.join(ROOT, "include", "daisyrec_b200.h")).read()
+
+
+def test_library_exports_and_binds_every_header_prototype():
     from daisyrec_b200 import _lib
-    hdr = open(os.path.join(ROOT, "include", "daisyrec_b200.h")).read()
+    hdr = _header()
     declared = set(re.findall(r"\b(drb_[a-z0-9_]+)\s*\(", hdr))
     assert declared, "no declarations parsed"
+    assert set(_lib.prototypes(hdr)) == declared, declared ^ set(_lib.prototypes(hdr))     # every drb_ prototype parses
     L = C.CDLL(_lib.so_path()) if os.path.exists(_lib.so_path()) else _lib.lib()
     for name in declared:
         assert hasattr(L, name), f"{name} declared in the header but not exported"
-    assert declared == set(_lib.SIGNATURES), declared ^ set(_lib.SIGNATURES)
-    assert _lib.lib().drb_version() >= 100
+    L = _lib.lib()
+    for name, (res, args) in _lib.signatures(hdr).items():
+        fn = getattr(L, name)
+        assert fn.restype is res and list(fn.argtypes) == args, name
+    assert L.drb_version() >= 100
+
+
+def test_header_scalars_bind_to_their_c_width_and_sign():
+    """Each scalar of a prototype binds to a ctypes type of the size and signedness its C name states; pointers stay pointers."""
+    from daisyrec_b200 import _lib
+    want = {"int": (4, True), "size_t": (C.sizeof(C.c_void_p), False), "unsigned long long": (8, False)}
+    seen = set()
+    for name, (ret, params) in _lib.prototypes(_header()).items():
+        for decl, t in [(ret, _lib.ctype(ret, name, ret=True))] + [(p, _lib.ctype(p, name)) for p in params]:
+            if "*" in decl:
+                assert t in (C.c_void_p, C.c_char_p) or issubclass(t, C._Pointer), (name, decl, t)
+                continue
+            base = decl.replace("const", "").strip()
+            seen.add(base)
+            if base in ("float", "double"):
+                assert C.sizeof(t) == (4 if base == "float" else 8) and t(0.5).value == 0.5, (name, decl, t)
+                continue
+            m = re.fullmatch(r"(u?)int(8|16|32|64)_t", base)
+            size, signed = (int(m[2]) // 8, not m[1]) if m else want[base]
+            assert C.sizeof(t) == size and (t(-1).value < 0) == signed, (name, decl, t)
+    assert {"int32_t", "int64_t", "uint32_t", "uint64_t", "size_t", "float", "double", "int"} <= seen, seen
+
+
+def test_header_parser_rejects_unknown_types():
+    from daisyrec_b200 import _lib
+    assert _lib.signatures("int drb_ok(unsigned long long *a, void *const *b, const drb_hyper *h);")["drb_ok"] == \
+        (C.c_int, [C.c_void_p, C.POINTER(C.c_void_p), C.POINTER(_lib.Hyper)])
+    for line in ("int drb_bad_arg(int32_t n, foo_t x);", "int drb_bad_arg(const bar_t *p);", "long drb_bad_ret(int32_t n);",
+                 "int drb_bad_arg(int32_t);"):
+        with pytest.raises(ValueError, match=re.escape(re.search(r"drb_\w+", line)[0])):
+            _lib.signatures(line)
+
+
+def test_hyper_matches_the_header_struct():
+    from daisyrec_b200 import _lib
+    body = re.search(r"typedef struct drb_hyper \{(.*?)\} drb_hyper;", _header(), re.S)[1]
+    body = re.sub(r"/\*.*?\*/", "", body, flags=re.S)
+    fields = []
+    for decl in filter(str.strip, body.split(";")):
+        ctype, names = re.fullmatch(r"\s*(\w+)\s+(.*?)\s*", decl, re.S).groups()
+        fields += [(n.strip(), _lib.ctype(ctype, "drb_hyper")) for n in names.split(",")]
+    assert _lib.Hyper._fields_ == fields
+
+
+def test_constants_come_from_the_header():
+    from daisyrec_b200 import _lib
+    from oracle import oracle as orc
+    d = _lib.defines(_header())
+    assert len(_lib.KPI_NAMES) == d["DRB_KPI_COUNT"] and [d["DRB_KPI_" + k.upper()] for k in _lib.KPI_NAMES] == list(range(8))
+    assert _lib.KPI_NAMES == orc.KPI_NAMES and _lib.OPT_KIND == orc.OPT_KIND and _lib.LOSS_KIND == orc.LOSS_KIND
+    assert (_lib.DRB_OK, _lib.DRB_ERR_INVALID, _lib.DRB_ERR_NAN_LOSS, _lib.DRB_ERR_EMPTY_SET, _lib.DRB_ERR_PEER,
+            _lib.DRB_ERR_NOT_PD) == (0, 1, 3, 4, 6, 7)
 
 
 def test_host_mt19937_entry_points_match_numpy():
