@@ -1025,3 +1025,155 @@ def slim_select(panel, topk, out=None):
     L.check(L.lib().drb_slim_select(_ptr(panel.lidx), _ptr(panel.w), _ptr(panel.nl), n, panel.begin, count, topk, _ptr(out.idx),
                                     _ptr(out.val), _ptr(out.cnt), _stream()))
     return out
+
+
+# ------------------------------------------------------------------ PureSVD
+def _round64(x):
+    return (x + 63) // 64 * 64
+
+
+class PureSvdX:
+    """X of PureSVD.fit on the device in fp64: the user-major CSR (row_ptr int64 [U+1], col int32 [nnz], val float64 [nnz]) and
+    the item-major CSR of X^T (t_ptr int64 [I+1], t_col int32 [nnz] users ascending, t_val float64 [nnz])."""
+
+    def __init__(self, row_ptr, col, val, t_ptr, t_col, t_val, user_num, item_num):
+        self.row_ptr, self.col, self.val = row_ptr, col, val
+        self.t_ptr, self.t_col, self.t_val = t_ptr, t_col, t_val
+        self.user_num, self.item_num = user_num, item_num
+
+    def operand(self, transposed):
+        """-> (row_ptr, col, val, n_rows) of X, or of X^T when ``transposed``."""
+        if transposed:
+            return self.t_ptr, self.t_col, self.t_val, self.item_num
+        return self.row_ptr, self.col, self.val, self.user_num
+
+
+def puresvd_csr(d_u, d_i, d_v, user_num, item_num):
+    """COO (int32 users, int32 items, float64 values) on the device -> PureSvdX: duplicates summed in fp64 in row order, as
+    csr_matrix((values, (u, i)), (U, I)) up to the order scipy gives three or more duplicates of one pair."""
+    _dev(d_v, torch.float64, "values")
+    row_ptr, col = csr_build(d_u, d_i, user_num, item_num)
+    col = col.contiguous()
+    seq_ptr, _, order = skipgram_group(d_u, user_num, 0)
+    t_ptr, t_col = csr_build(d_i, d_u, item_num, user_num)
+    nnz, dev = col.numel(), d_u.device
+    assert t_col.numel() == nnz
+    t_col = t_col.contiguous()
+    val = torch.empty(max(nnz, 1), dtype=torch.float64, device=dev)
+    t_val = torch.empty(max(nnz, 1), dtype=torch.float64, device=dev)
+    L.check(L.lib().drb_puresvd_csr(_ptr(seq_ptr), _ptr(order), _ptr(d_i), _ptr(d_v), user_num, item_num, _ptr(row_ptr), _ptr(col),
+                                    nnz, _ptr(t_ptr), _ptr(t_col), _ptr(val), _ptr(t_val), _stream()))
+    return PureSvdX(row_ptr, col, val[:nnz], t_ptr, t_col, t_val[:nnz], user_num, item_num)
+
+
+def puresvd_panel(rows, l, device):
+    """A zero fp64 panel [rows rounded up to 64, l rounded up to 64] (the layout of every PureSVD panel)."""
+    return torch.zeros((_round64(rows), _round64(l)), dtype=torch.float64, device=device)
+
+
+def puresvd_spmm(A, Z, l, Y):
+    """Y[r, :l] = sum_j A[r, j] Z[j, :l] for A = (row_ptr, col, val, n_rows); Y's columns l .. ld are written 0."""
+    row_ptr, col, val, n_rows = A
+    _dev(Z, torch.float64, "Z"); _dev(Y, torch.float64, "Y")
+    L.check(L.lib().drb_puresvd_spmm(_ptr(row_ptr), _ptr(col), _ptr(val), n_rows, _ptr(Z), l, Y.shape[1], _ptr(Y), _stream()))
+    return Y
+
+
+def puresvd_orth_workspace(m, l, device):
+    return torch.empty(L.lib().drb_puresvd_orth_workspace_bytes(m, _round64(l)), dtype=torch.uint8, device=device)
+
+
+def puresvd_orth(Y, m, l, ws=None, want_r=False):
+    """In place: the first m rows of the panel Y -> Q of shifted CholeskyQR3 (Y = Q R).  -> R fp64 [ld, ld] (upper, padded block
+    identity) when ``want_r``.  numpy.linalg.LinAlgError when the panel is numerically rank deficient."""
+    _dev(Y, torch.float64, "Y")
+    ld = Y.shape[1]
+    ws = puresvd_orth_workspace(m, l, Y.device) if ws is None else ws
+    R = torch.empty((ld, ld), dtype=torch.float64, device=Y.device) if want_r else None
+    L.check(L.lib().drb_puresvd_orth(_ptr(Y), m, l, ld, _ptr(ws), None if R is None else _ptr(R), _stream()))
+    return R
+
+
+def puresvd_small_svd(R, l):
+    """One-sided Jacobi SVD of R[:l, :l]^T -> (s fp64 [l], UT fp64 [ld, ld], VT fp64 [ld, ld]): rows j of UT / VT are the left /
+    right singular vectors of R^T for s[j], unsorted."""
+    _dev(R, torch.float64, "R")
+    ld = R.shape[1]
+    s = torch.empty(l, dtype=torch.float64, device=R.device)
+    UT = torch.empty((ld, ld), dtype=torch.float64, device=R.device)
+    VT = torch.empty((ld, ld), dtype=torch.float64, device=R.device)
+    L.check(L.lib().drb_puresvd_small_svd(_ptr(R), l, ld, _ptr(s), _ptr(UT), _ptr(VT), _stream()))
+    return s, UT, VT
+
+
+def puresvd_factors(Q, m, Qb, n, l, s, UT, VT, transposed, k, user_num, item_num):
+    """U_A = Q Ur, V_A = Q_b Vr for the k largest sigma -> (user_vec fp64 [U, k], item_vec fp64 [I, k], sigma fp64 [l] sorted)."""
+    ld = Q.shape[1]
+    dev = Q.device
+    ws = torch.empty(L.lib().drb_puresvd_factors_workspace_bytes(m, n, ld, k), dtype=torch.uint8, device=dev)
+    P = torch.empty((user_num, k), dtype=torch.float64, device=dev)
+    V = torch.empty((item_num, k), dtype=torch.float64, device=dev)
+    sigma = torch.empty(l, dtype=torch.float64, device=dev)
+    L.check(L.lib().drb_puresvd_factors(_ptr(Q), m, _ptr(Qb), n, l, ld, _ptr(s), _ptr(UT), _ptr(VT), int(bool(transposed)), k,
+                                        _ptr(ws), _ptr(P), _ptr(V), _ptr(sigma), _stream()))
+    return P, V, sigma
+
+
+def puresvd_fit(X, omega, factors, n_iter, transposed, mark=None):
+    """randomized_svd's sequence on the device: Omega (host fp64 [min(U, I), l]) -> n_iter rounds of Y = orth(A Z),
+    Z = orth(A^T Y), then Q = orth(A Z), Q_b R = A^T Q, the SVD of R^T and the factors.  A = X^T when ``transposed``.
+    ``mark(phase)`` is called after each phase (for timing).  -> (user_vec, item_vec, sigma)."""
+    dev = X.val.device
+    mark = mark or (lambda phase: None)
+    n, l = omega.shape
+    A, At = X.operand(transposed), X.operand(not transposed)
+    m = A[3]
+    Z = puresvd_panel(n, l, dev)
+    Z[:n, :l] = torch.from_numpy(np.ascontiguousarray(omega, np.float64)).to(dev)
+    Y = puresvd_panel(m, l, dev)
+    ws_m, ws_n = puresvd_orth_workspace(m, l, dev), puresvd_orth_workspace(n, l, dev)
+    mark("upload")
+    for _ in range(n_iter):
+        puresvd_spmm(A, Z, l, Y); mark("spmm")
+        puresvd_orth(Y, m, l, ws_m); mark("orth")
+        puresvd_spmm(At, Y, l, Z); mark("spmm")
+        puresvd_orth(Z, n, l, ws_n); mark("orth")
+    puresvd_spmm(A, Z, l, Y); mark("spmm")
+    puresvd_orth(Y, m, l, ws_m); mark("orth")
+    puresvd_spmm(At, Y, l, Z); mark("spmm")
+    R = puresvd_orth(Z, n, l, ws_n, want_r=True); mark("orth")
+    del ws_m, ws_n
+    s, UT, VT = puresvd_small_svd(R, l); mark("small_svd")
+    out = puresvd_factors(Y, m, Z, n, l, s, UT, VT, transposed, factors, X.user_num, X.item_num); mark("factors")
+    return out
+
+
+def puresvd_scores(user_vec, item_vec, users, cands=None):
+    """-> fp64 [n, C] user_vec[u] . item_vec[c] for ``cands`` int64 [n, C], or [n, I] over every item."""
+    _dev(user_vec, torch.float64, "user_vec"); _dev(item_vec, torch.float64, "item_vec"); _dev(users, torch.int64, "users")
+    n, k = users.numel(), user_vec.shape[1]
+    cnum = item_vec.shape[0] if cands is None else _dev(cands, torch.int64, "cands").shape[1]
+    sc = torch.empty((n, cnum), dtype=torch.float64, device=users.device)
+    L.check(L.lib().drb_puresvd_scores(_ptr(user_vec), _ptr(item_vec), k, _ptr(users), n, None if cands is None else _ptr(cands),
+                                       cnum, _ptr(sc), _stream()))
+    return sc
+
+
+def puresvd_rank(user_vec, item_vec, users, cands, topk, scores=False):
+    """-> int64 [n, topk] candidate ids by (score descending, candidate position ascending) (and the scores when asked)."""
+    sc = puresvd_scores(user_vec, item_vec, users, cands)
+    out = _itemknn_topk(sc, cands, topk)
+    return (out, sc) if scores else out
+
+
+def puresvd_full_rank(user_vec, item_vec, users, topk, scores=False):
+    """-> int64 [n, topk] item ids by (score descending, id ascending) over every item (and the scores when asked)."""
+    sc = puresvd_scores(user_vec, item_vec, users)
+    out = _itemknn_topk(sc, None, topk)
+    return (out, sc) if scores else out
+
+
+def puresvd_predict(user_vec, item_vec, users, items):
+    """-> fp64 [n]: user_vec[u] . item_vec[i] per (u, i) pair."""
+    _dev(items, torch.int64, "items")
+    return puresvd_scores(user_vec, item_vec, users, items.reshape(-1, 1).contiguous()).reshape(-1)

@@ -589,6 +589,41 @@ int drb_slim_solve(const double *d_G, int32_t item_num, int32_t begin, int32_t c
 int drb_slim_select(const int32_t *d_lidx, const double *d_w, const int32_t *d_nl, int32_t item_num, int32_t begin, int32_t count,
                     int32_t topk, int32_t *d_nbr_idx, float *d_nbr_val, int32_t *d_nbr_cnt, void *stream);
 
+/* ---- PureSVD: daisy/model/PureSVDRecommender.py (sklearn randomized_svd), csrc/puresvd.cu ----------------------------------
+ * All fp64, every sum in a fixed order: two fits are bitwise equal.  A panel is row-major [rows padded to 64, ld] with
+ * ld = l rounded up to 64; its padded rows and columns are zero.
+ * drb_puresvd_csr         X = csr_matrix((rating, (user, item)), (U, I)) in fp64 (:53-59): d_val[k] = the sum, in row order,
+ *                         of the COO values of slot k of the drb_csr_build CSR (d_row_ptr, d_col); d_seq_ptr / d_order as for
+ *                         drb_ease_csr.  (scipy sums three or more duplicates of a pair in an order of its own sort.)  X^T:
+ *                         d_t_ptr / d_t_col = drb_csr_build of the (item, user) pairs; d_t_val[k] = the value of that pair in X.
+ * drb_puresvd_spmm        d_Y[r, :] = sum_j A[r, j] d_Z[j, :] for the n_rows rows of one CSR (X or X^T); columns l .. ld of
+ *                         d_Y are written 0, padded rows are left as they are.  Each row summed in CSR order.
+ * drb_puresvd_orth        shifted CholeskyQR3 of d_Y [m, l] in place (Y = Q R, Q^T Q = I); d_R (ld x ld, optional) receives
+ *                         R (upper, padded block identity).  DRB_ERR_NOT_PD when the panel is numerically rank deficient (a
+ *                         Cholesky pivot <= l u max_j W_jj).  d_ws: drb_puresvd_orth_workspace_bytes(m, ld).  Synchronises.
+ * drb_puresvd_small_svd   one-sided Jacobi SVD of R^T for d_R upper [l, l] (leading dimension ld) in one CTA: d_s [l] the
+ *                         singular values, d_UT / d_VT [ld, ld] rows j = the left / right singular vectors of R^T, unsorted.
+ * drb_puresvd_factors     d_Q [m] = Q of A, d_Qb [n] = Q_b of A^T: U_A = Q Ur, V_A = Q_b Vr for the k largest sigma (index
+ *                         ascending on ties) -> d_sigma [l] sorted descending, d_user_vec [U, k] with every column's largest-
+ *                         magnitude entry (first row on ties) positive, d_item_vec [I, k] scaled by sigma.  transposed != 0:
+ *                         A = X^T (the user side is V_A).  d_ws: drb_puresvd_factors_workspace_bytes(m, n, ld, k).
+ * drb_puresvd_scores      d_scores [n_users, cand_num] = user_vec[u] . item_vec[c] over k, for the rows' candidates d_cands
+ *                         int64 [n_users, cand_num], or every item (d_cands NULL, cand_num = item_num). */
+int drb_puresvd_csr(const int64_t *d_seq_ptr, const int32_t *d_order, const int32_t *d_coo_i, const double *d_coo_v,
+                    int32_t user_num, int32_t item_num, const int64_t *d_row_ptr, const int32_t *d_col, int64_t nnz,
+                    const int64_t *d_t_ptr, const int32_t *d_t_col, double *d_val, double *d_t_val, void *stream);
+int drb_puresvd_spmm(const int64_t *d_row_ptr, const int32_t *d_col, const double *d_val, int32_t n_rows, const double *d_Z,
+                     int32_t l, int32_t ld, double *d_Y, void *stream);
+size_t drb_puresvd_orth_workspace_bytes(int64_t m, int32_t ld);
+int drb_puresvd_orth(double *d_Y, int64_t m, int32_t l, int32_t ld, void *d_ws, double *d_R, void *stream);
+int drb_puresvd_small_svd(const double *d_R, int32_t l, int32_t ld, double *d_s, double *d_UT, double *d_VT, void *stream);
+size_t drb_puresvd_factors_workspace_bytes(int64_t m, int64_t n, int32_t ld, int32_t k);
+int drb_puresvd_factors(const double *d_Q, int64_t m, const double *d_Qb, int64_t n, int32_t l, int32_t ld, const double *d_s,
+                        const double *d_UT, const double *d_VT, int32_t transposed, int32_t k, void *d_ws, double *d_user_vec,
+                        double *d_item_vec, double *d_sigma, void *stream);
+int drb_puresvd_scores(const double *d_user_vec, const double *d_item_vec, int32_t k, const int64_t *d_users, int64_t n_users,
+                       const int64_t *d_cands, int32_t cand_num, double *d_scores, void *stream);
+
 /* ---- evaluation: calc_ranking_results / Metric.run ------------------------------------------------
  * daisy/utils/metrics.py:18-57 (cut-off loop), :59-96 (dispatch), :98-251 (the KPIs).
  * d_preds: rank()'s float32 [n_users, ld] output; ground truth as CSR aligned with its rows
