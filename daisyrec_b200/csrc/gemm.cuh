@@ -16,6 +16,12 @@ int gemm_nn(int dtype, long long M, int N, int K, const float *A, long long lda,
 // C[N,M] += (A[K,M]^T B[K,N])^T   (weight gradient [out, in] += dZ^T X, computed with the wide dimension on the MMA rows; split-K)
 int gemm_tn_acc_t(int dtype, long long M, int N, int K, const float *A, long long lda, const float *B, long long ldb, float *C,
                   long long ldc, cudaStream_t st);
+// C[M,N] = A[K,M]^T B[K,N]        (weight gradient written, not accumulated: fp32, each output summed over k in order)
+int gemm_tn(long long M, int N, int K, const float *A, long long lda, const float *B, long long ldb, float *C, long long ldc,
+            cudaStream_t st);
+// C + z (M ldc) = A[M, Kz] B[Kz, N] for the z-th of `slices` equal k ranges (fp32; the caller sums the slices in a fixed order)
+int gemm_nn_slices(long long M, int N, int K, const float *A, long long lda, const float *B, long long ldb, float *C,
+                   long long ldc, int slices, cudaStream_t st);
 // gb[n] += sum_m dZ[m, n]          (bias gradient, N <= 256)
 int colsum_acc(const float *dZ, long long M, int N, float *gb, cudaStream_t st);
 // the same over the 2B rows of a pairwise step, each pos row m added to its neg row B + m first

@@ -106,6 +106,7 @@ static size_t carve_neumf(void *base, const NeumfDims &d, int opt, long long max
 //   TB = false: B(k,n) = B[k*ldb + n]      TB = true: B(k,n) = B[n*ldb + k]
 //   EPI 0: C = acc   1: C = relu(acc + bias[n])   2: C = acc * (ref(m,n) > 0)   3: atomicAdd(C, acc) (split-K over grid.z)
 //   EPI 4: atomicAdd(C^T, acc): the product is accumulated into the transposed matrix C[n*ldc + m] (split-K)
+//   EPI 5: C + z * ldref = acc: split-K into per-slice matrices (grid.z slices, no atomics; the caller sums them in order)
 template <bool TA, bool TB, int EPI>
 __global__ void __launch_bounds__(256) sgemm_kernel(int M, int N, int K, const float *__restrict__ A, long long lda,
                                                     const float *__restrict__ B, long long ldb, float *__restrict__ C,
@@ -169,6 +170,7 @@ __global__ void __launch_bounds__(256) sgemm_kernel(int M, int N, int K, const f
             if (EPI == 2) { v = (ref[m * ldref + n] > 0.f) ? v * alpha : 0.f; }
             if (EPI == 3) atomicAdd(C + m * ldc + n, v);
             else if (EPI == 4) atomicAdd(C + (long long)n * ldc + m, v);   // transposed accumulate: C^T += acc
+            else if (EPI == 5) C[(long long)blockIdx.z * ldref + m * ldc + n] = v;
             else C[m * ldc + n] = v;
         }
     }
@@ -176,12 +178,16 @@ __global__ void __launch_bounds__(256) sgemm_kernel(int M, int N, int K, const f
 
 template <bool TA, bool TB, int EPI>
 static int launch_sgemm(long long M, int N, int K, const float *A, long long lda, const float *B, long long ldb, float *C,
-                        long long ldc, const float *bias, const float *ref, long long ldref, cudaStream_t st, float alpha = 1.f)
+                        long long ldc, const float *bias, const float *ref, long long ldref, cudaStream_t st, float alpha = 1.f,
+                        int slices = 0)
 {
     if (M <= 0 || N <= 0 || K <= 0) return DRB_OK;
     dim3 grid((unsigned)((M + 63) / 64), (unsigned)((N + 63) / 64), 1);
     int k_chunk = K;
-    if (EPI >= 3) {   // split-K so that the tiny [out x in] result still fills the machine
+    if (EPI == 5) {   // a fixed number of slices, chosen by the caller: the same shapes always split the same way
+        k_chunk = (int)(((K + slices - 1) / slices + 15) / 16 * 16);
+        grid.z = (unsigned)((K + k_chunk - 1) / k_chunk);
+    } else if (EPI >= 3) {   // split-K so that the tiny [out x in] result still fills the machine
         long long tiles = (long long)grid.x * grid.y;
         long long want = ((long long)sm_count() * 4 + tiles - 1) / tiles;          // chunks wanted for occupancy
         long long max_chunks = (K + 2047) / 2048;                                   // >= 2048 rows per chunk
@@ -561,6 +567,17 @@ int gemm_tn_acc_t(int dtype, long long M, int N, int K, const float *A, long lon
                   long long ldc, cudaStream_t st)
 {
     return launch_gemm<true, false, 4>(dtype, M, N, K, A, lda, B, ldb, C, ldc, nullptr, nullptr, 0, st);
+}
+int gemm_tn(long long M, int N, int K, const float *A, long long lda, const float *B, long long ldb, float *C, long long ldc,
+            cudaStream_t st)
+{
+    return launch_sgemm<true, false, 0>(M, N, K, A, lda, B, ldb, C, ldc, nullptr, nullptr, 0, st);
+}
+int gemm_nn_slices(long long M, int N, int K, const float *A, long long lda, const float *B, long long ldb, float *C,
+                   long long ldc, int slices, cudaStream_t st)
+{
+    DRB_REQUIRE(slices >= 1 && slices <= K, "gemm_nn_slices: slices=%d for K=%d", slices, K);
+    return launch_sgemm<false, false, 5>(M, N, K, A, lda, B, ldb, C, ldc, nullptr, nullptr, M * ldc, st, 1.f, slices);
 }
 int colsum_acc(const float *dZ, long long M, int N, float *gb, cudaStream_t st)
 {

@@ -81,14 +81,14 @@ def epoch_permutation(n, shuffle, generator=None, seed=None):
     return torch.randperm(n, generator=g)
 
 
-def loader_plan(train_loader):
-    """Decode a DataLoader into (triples ndarray, batch_size, shuffle, drop_last, generator), or None when it is not the
-    plain ``DataLoader(BasicDataset(int[T,3]), batch_size, shuffle)`` of run_examples/test.py:93-94 (then fit() falls back
-    to iterating it batch by batch)."""
+def loader_plan(train_loader, rows_ok=lambda data: data.ndim == 2 and data.shape[1] == 3):
+    """Decode a DataLoader into (rows ndarray, batch_size, shuffle, drop_last, generator), or None when it is not the
+    plain ``DataLoader(BasicDataset(int[T,3]), batch_size, shuffle)`` of run_examples/test.py:93-94 -- or another dataset whose
+    ``.data`` passes ``rows_ok`` -- (then fit() falls back to iterating it batch by batch)."""
     ds = getattr(train_loader, 'dataset', None)
     data = getattr(ds, 'data', None)
     bs = getattr(train_loader, 'batch_size', None)
-    if not isinstance(data, np.ndarray) or data.ndim != 2 or data.shape[1] != 3 or bs is None:
+    if not isinstance(data, np.ndarray) or not rows_ok(data) or bs is None:
         return None
     sampler = getattr(train_loader, 'sampler', None)
     if not isinstance(getattr(train_loader, 'batch_sampler', None), BatchSampler):

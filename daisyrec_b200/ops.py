@@ -1177,3 +1177,121 @@ def puresvd_predict(user_vec, item_vec, users, items):
     """-> fp64 [n]: user_vec[u] . item_vec[i] per (u, i) pair."""
     _dev(items, torch.int64, "items")
     return puresvd_scores(user_vec, item_vec, users, items.reshape(-1, 1).contiguous()).reshape(-1)
+
+
+# ------------------------------------------------------------------ Multi-VAE
+def _vae_hidden(hidden):
+    return (C.c_int32 * max(1, len(hidden)))(*[int(h) for h in hidden]), len(hidden)
+
+
+def vae_param_count(item_num, hidden, latent_dim):
+    h, nh = _vae_hidden(hidden)
+    return int(L.lib().drb_vae_param_count(item_num, h, nh, latent_dim))
+
+
+class VaeInput:
+    """The input rows of every user (drb_vae_input_csr): row_ptr int64 [U + 1], col int32 / val fp32 [nnz] on the device."""
+
+    def __init__(self, hist_id, hist_val, item_num):
+        _dev(hist_id, torch.int64, "history_item_id")
+        _dev(hist_val, torch.float32, "history_item_value")
+        U, Lh = hist_id.shape
+        self.user_num, self.item_num = int(U), int(item_num)
+        self.row_ptr = torch.empty(U + 1, dtype=torch.int64, device=hist_id.device)
+        nnz = C.c_int64()
+        L.check(L.lib().drb_vae_input_csr(_ptr(hist_id), _ptr(hist_val), U, Lh, item_num, _ptr(self.row_ptr), None, None,
+                                          C.byref(nnz), _stream()))
+        self.col = torch.empty(max(1, nnz.value), dtype=torch.int32, device=hist_id.device)
+        self.val = torch.empty(max(1, nnz.value), dtype=torch.float32, device=hist_id.device)
+        L.check(L.lib().drb_vae_input_csr(_ptr(hist_id), _ptr(hist_val), U, Lh, item_num, _ptr(self.row_ptr), _ptr(self.col),
+                                          _ptr(self.val), C.byref(nnz), _stream()))
+        self.nnz = nnz.value
+        self.max_row_len = int((self.row_ptr[1:] - self.row_ptr[:-1]).max().item())
+
+
+VAE_MAX_ROWS = 32768       # users per step / scoring pass (drb_vae_train_steps)
+
+
+class VaeWorkspace:
+    """opt: 'sgd' / 'adam', or None for a scoring workspace (no gradient or optimiser state).  The nonzero scratch holds
+    max_rows rows of the input's longest row, so no batch of at most max_rows users outgrows it."""
+
+    def __init__(self, item_num, hidden, latent_dim, opt, max_rows, max_row_len, device):
+        self.I, self.hidden, self.lat = int(item_num), [int(h) for h in hidden], int(latent_dim)
+        self.max_rows, self.max_row_len = int(max_rows), int(max_row_len)
+        if not 1 <= self.max_rows <= VAE_MAX_ROWS:
+            raise ValueError(f"Multi-VAE: a step takes 1 .. {VAE_MAX_ROWS} users, got {self.max_rows}")
+        self.opt = -1 if opt is None else (L.OPT_SGD if opt == "sgd" else L.OPT_ADAM)
+        self._h = _vae_hidden(self.hidden)
+        nbytes = L.lib().drb_vae_workspace_bytes(self.I, *self._h, self.lat, self.opt, self.max_rows, self.max_row_len)
+        if nbytes == 0:
+            raise ValueError("Multi-VAE: need 1 <= item_num <= 2^20, at most 8 positive hidden sizes and latent_dim >= 2")
+        self.buf = torch.empty(nbytes, dtype=torch.uint8, device=device)
+        L.check(L.lib().drb_vae_workspace_init(_ptr(self.buf), self.I, *self._h, self.lat, self.opt, self.max_rows,
+                                               self.max_row_len, _stream()))
+
+    def state_bytes(self):
+        """bytes of the header, gradient and optimiser state at the start of the workspace (the library's carve)"""
+        a = lambda n: (n + 255) // 256 * 256  # noqa: E731
+        nW = vae_param_count(self.I, self.hidden, self.lat)
+        return 256 + {-1: 0, L.OPT_SGD: 1, L.OPT_ADAM: 3}[self.opt] * a(4 * nW)
+
+    def grown(self, max_rows):
+        """a workspace for up to max_rows users carrying this one's gradient and optimiser state"""
+        new = VaeWorkspace(self.I, self.hidden, self.lat, {-1: None, L.OPT_SGD: "sgd", L.OPT_ADAM: "adam"}[self.opt],
+                           max_rows, self.max_row_len, self.buf.device)
+        n = self.state_bytes()
+        new.buf[:n].copy_(self.buf[:n])
+        return new
+
+    def dims(self):
+        return (self.I, *self._h, self.lat, self.opt, self.max_rows, self.max_row_len)
+
+
+def vae_keep_words(batch, item_num):
+    """uint32 words of one step's bit-packed [batch, item_num] keep mask."""
+    return (batch * item_num + 31) // 32
+
+
+def vae_train_steps(W, ws, inp, users, batch, first_step, n_steps, hp, adam_step0=0, apply=True, training=True, update0=0,
+                    total_anneal_steps=0, anneal_cap=0.2, dropout=0.0, seed=0, keep_bits=None, eps=None, check=True):
+    """users: int64 CUDA tensor of the epoch's batch rows; keep_bits (int32 [n_steps * vae_keep_words]) and eps (fp32
+    [n_steps, batch, latent_dim // 2]): host draws, both or neither (drb_vae_train_steps)."""
+    _dev(W, torch.float32, "W")
+    _dev(users, torch.int64, "users")
+    if (keep_bits is None) != (eps is None) and training and dropout > 0.0:
+        raise ValueError("keep_bits and eps are drawn together")
+    if keep_bits is not None:
+        _dev(keep_bits, torch.int32, "keep_bits")
+        if keep_bits.numel() < n_steps * vae_keep_words(batch, ws.I):
+            raise ValueError("keep_bits too short for n_steps batches")
+    if eps is not None:
+        _dev(eps, torch.float32, "eps")
+        if eps.numel() < n_steps * batch * (ws.lat // 2):
+            raise ValueError("eps too short for n_steps batches")
+    return _train_steps(
+        L.lib().drb_vae_train_steps, n_steps, W.device, check, _ptr(W), _ptr(ws.buf), *ws.dims(), _ptr(inp.row_ptr),
+        _ptr(inp.col), _ptr(inp.val), _ptr(users), users.numel(), batch, first_step, n_steps, C.byref(hp), adam_step0,
+        1 if apply else 0, 1 if training else 0, int(update0), int(total_anneal_steps), C.c_double(anneal_cap),
+        C.c_float(dropout), C.c_uint64(seed), None if keep_bits is None else _ptr(keep_bits), None if eps is None else _ptr(eps))
+
+
+def vae_scores(W, ws, inp, users, cands=None):
+    """eval-mode logits: [n, C] of the candidates (int64 [n, C]) or [n, item_num] of every item."""
+    _dev(users, torch.int64, "users")
+    if cands is not None:
+        _dev(cands, torch.int64, "cands")
+    n, cnt = users.numel(), (cands.shape[1] if cands is not None else ws.I)
+    out = torch.empty((n, cnt), dtype=torch.float32, device=W.device)
+    L.check(L.lib().drb_vae_scores(_ptr(W), _ptr(ws.buf), *ws.dims(), _ptr(inp.row_ptr), _ptr(inp.col), _ptr(inp.val),
+                                   _ptr(users), n, None if cands is None else _ptr(cands), cnt, _ptr(out), _stream()))
+    return out
+
+
+def vae_philox_draws(seed, step, dropout, rows, cols, half, device):
+    """test hook: the 'philox' engine's keep bits uint8 [rows, cols] and normals fp32 [rows, half] of one step"""
+    keep = torch.empty((rows, cols), dtype=torch.uint8, device=device)
+    eps = torch.empty((rows, half), dtype=torch.float32, device=device)
+    L.check(L.lib().drb_vae_philox_draws(C.c_uint64(seed), step, C.c_float(dropout), rows, cols, half, _ptr(keep), _ptr(eps),
+                                         _stream()))
+    return keep, eps

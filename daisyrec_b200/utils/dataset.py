@@ -15,7 +15,7 @@ def get_dataloader(ds, batch_size, shuffle, num_workers=4):
 
 
 def _bulk(ds):
-    return isinstance(ds, (BasicDataset, CandidatesDataset))
+    return isinstance(ds, (BasicDataset, CandidatesDataset, AEDataset))
 
 
 class BasicDataset(Dataset):
@@ -46,3 +46,18 @@ class CandidatesDataset(Dataset):
     def __getitem__(self, index):
         u, c = self.data[index]
         return torch.tensor(u), torch.tensor(c)
+
+
+class AEDataset(Dataset):
+    """The distinct users (or items) of the train set in order of first appearance, for the autoencoders
+    (daisy/utils/dataset.py:40-58)."""
+
+    def __init__(self, train_set, yield_col='user'):
+        super().__init__()
+        self.data = train_set[yield_col].unique()
+
+    def __len__(self):
+        return len(self.data)
+
+    def __getitem__(self, index):
+        return self.data[index]

@@ -107,3 +107,32 @@ def build_candidates_set(test_ur, train_ur, config, drop_past_inter=True):
             samples = np.concatenate((picked[lo:hi].astype(np.int64), gts[k]), axis=None)
         test_ucands.append([u, samples])
     return test_u, test_ucands
+
+
+def get_history_matrix(df, config, row='user', use_config_value_name=False):
+    """daisy/utils/utils.py:87-123, vectorised: (ids int64 [rows, max_len], values fp32 [rows, max_len], lengths int64 [rows]).
+    Row r lists its interactions in DataFrame order; the padding is (0, 0.0)."""
+    logger = config['logger']
+    assert row in df.columns, f'invalid name {row}: not in columns of history dataframe'
+    uid_name, iid_name = config['UID_NAME'], config['IID_NAME']
+    user_ids, item_ids = np.asarray(df[uid_name].values), np.asarray(df[iid_name].values)
+    values = np.ones(len(df)) if not use_config_value_name else np.asarray(df[config['INTER_NAME']].values)
+    user_num, item_num = config['user_num'], config['item_num']
+    if row == 'user':
+        row_num, max_col_num, row_ids, col_ids = user_num, item_num, user_ids, item_ids
+    else:
+        row_num, max_col_num, row_ids, col_ids = item_num, user_num, item_ids, user_ids
+    row_ids = row_ids.astype(np.int64)
+    history_len = np.bincount(row_ids, minlength=row_num).astype(np.int64)
+    col_num = int(history_len.max()) if len(history_len) else 0
+    if col_num > max_col_num * 0.2:
+        logger.info(f'Max value of {row}\'s history interaction records has reached: {col_num / max_col_num * 100:.4f}% of the total.')
+    order = np.argsort(row_ids, kind='stable')
+    starts = np.concatenate([[0], np.cumsum(history_len)[:-1]])
+    slot = np.empty(len(row_ids), dtype=np.int64)
+    slot[order] = np.arange(len(row_ids)) - np.repeat(starts, history_len)
+    history_matrix = np.zeros((row_num, col_num), dtype=np.int64)
+    history_value = np.zeros((row_num, col_num))
+    history_matrix[row_ids, slot] = col_ids
+    history_value[row_ids, slot] = values
+    return torch.LongTensor(history_matrix), torch.FloatTensor(history_value), torch.LongTensor(history_len)

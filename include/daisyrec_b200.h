@@ -624,6 +624,54 @@ int drb_puresvd_factors(const double *d_Q, int64_t m, const double *d_Qb, int64_
 int drb_puresvd_scores(const double *d_user_vec, const double *d_item_vec, int32_t k, const int64_t *d_users, int64_t n_users,
                        const int64_t *d_cands, int32_t cand_num, double *d_scores, void *stream);
 
+/* ---- Multi-VAE: daisy/model/VAECFRecommender.py (VAECF), csrc/vae.cu ------------------------------------------------------
+ * fp32 on CUDA cores, every sum in a fixed order and no floating-point atomics: two fits are bitwise equal.
+ * Layers (:50-69): encoder [I] + hidden + [lat], decoder [lat / 2] + reversed(hidden) + [I], Tanh between, none after the last;
+ * h_hidden[n_hidden] (host) are the hidden widths, latent_dim >= 2.  d_W: one flat fp32 block, encoder then decoder, per layer W
+ * [out, in] then b [out], except the first encoder weight, stored item-major [I, hidden[0]] (nn.Linear's weight transposed).
+ * drb_vae_input_csr     get_user_rating_matrix (AbstractRecommender.py:147-158) of every user as a CSR: for each (u, item) the
+ *                       value of the LAST slot of row u of the padded history (d_hist_id int64 / d_hist_val fp32 [U, max_len],
+ *                       utils.py:87-123) that names the item, as index_put_ leaves it on the CPU; zero values are absent; entries
+ *                       in slot order.  Call with d_col = NULL first: d_row_ptr [U + 1] and *h_nnz; then again with d_col / d_val
+ *                       [*h_nnz].  Synchronises.
+ * drb_vae_train_steps   calc_loss :92-110 + backward + optimizer.step for steps [first_step, first_step + n_steps) of batch rows
+ *                       d_users [n] (int64); apply = 0: the loss of one batch, nothing updated.  training != 0 is train mode:
+ *                       F.dropout(dropout) (:81) and z = mu + eps exp(logvar / 2) (:71-77); else eval mode (z = mu).  Step s
+ *                       anneals with min(anneal_cap, (update0 + s + 1) / total_anneal_steps), or anneal_cap when
+ *                       total_anneal_steps <= 0 (:97-100).  d_keep_bits (with d_eps): per step the bit-packed [B, I] keep mask
+ *                       torch draws (bit b * I + item), and d_eps [B, lat / 2] the randn_like draws (parity mode, full batches
+ *                       only); both NULL: Philox keep bits at the nonzeros and Philox normals, keyed by seed and adam_step0 + s.
+ *                       DRB_ERR_NAN_LOSS as drb_mf_bpr_train_steps.  max_rows >= batch (<= 32768).  max_row_len: the longest
+ *                       input row (drb_vae_input_csr), which sizes the nonzero scratch to max_rows rows of it; a longer row
+ *                       makes the call fail with DRB_ERR_INVALID and writes nothing out of bounds.  opt = -1 lays out a
+ *                       scoring workspace (no gradient or optimiser state), which drb_vae_train_steps refuses.
+ * drb_vae_scores        forward() in eval mode (:79-90): d_scores [n_users, cand_num] = the logits of the rows' candidates
+ *                       d_cands int64 [n_users, cand_num] (rank :121-138, predict :112-119; one warp dot per candidate), or of
+ *                       every item (d_cands NULL, cand_num = item_num: full_rank :140-145).  Feed to drb_topk_from_scores.
+ *                       Synchronises (reads the workspace status).
+ * drb_vae_philox_draws  test hook: the 'philox' keep bits d_keep [rows, cols] (1 = kept) and normals d_eps [rows, half] of one
+ *                       step, from the device functions drb_vae_train_steps uses. */
+int64_t drb_vae_param_count(int32_t item_num, const int32_t *h_hidden, int32_t n_hidden, int32_t latent_dim);
+size_t drb_vae_workspace_bytes(int32_t item_num, const int32_t *h_hidden, int32_t n_hidden, int32_t latent_dim, int32_t opt,
+                               int64_t max_rows, int32_t max_row_len);
+int drb_vae_workspace_init(void *d_ws, int32_t item_num, const int32_t *h_hidden, int32_t n_hidden, int32_t latent_dim,
+                           int32_t opt, int64_t max_rows, int32_t max_row_len, void *stream);
+int drb_vae_input_csr(const int64_t *d_hist_id, const float *d_hist_val, int32_t user_num, int32_t max_len, int32_t item_num,
+                      int64_t *d_row_ptr, int32_t *d_col, float *d_val, int64_t *h_nnz, void *stream);
+int drb_vae_train_steps(float *d_W, void *d_ws, int32_t item_num, const int32_t *h_hidden, int32_t n_hidden, int32_t latent_dim,
+                        int32_t opt, int64_t max_rows, int32_t max_row_len, const int64_t *d_row_ptr, const int32_t *d_col,
+                        const float *d_val, const int64_t *d_users, int64_t n, int64_t batch, int64_t first_step, int64_t n_steps,
+                        const drb_hyper *hyper, int64_t adam_step0, int32_t apply, int32_t training, int64_t update0,
+                        int64_t total_anneal_steps, double anneal_cap, float dropout, uint64_t seed,
+                        const uint32_t *d_keep_bits, const float *d_eps, double *d_step_loss, int32_t sync_and_check,
+                        int64_t *nan_step, void *stream);
+int drb_vae_scores(const float *d_W, void *d_ws, int32_t item_num, const int32_t *h_hidden, int32_t n_hidden, int32_t latent_dim,
+                   int32_t opt, int64_t max_rows, int32_t max_row_len, const int64_t *d_row_ptr, const int32_t *d_col,
+                   const float *d_val, const int64_t *d_users, int64_t n_users, const int64_t *d_cands, int32_t cand_num,
+                   float *d_scores, void *stream);
+int drb_vae_philox_draws(uint64_t seed, int64_t step, float dropout, int32_t rows, int32_t cols, int32_t half, uint8_t *d_keep,
+                         float *d_eps, void *stream);
+
 /* ---- evaluation: calc_ranking_results / Metric.run ------------------------------------------------
  * daisy/utils/metrics.py:18-57 (cut-off loop), :59-96 (dispatch), :98-251 (the KPIs).
  * d_preds: rank()'s float32 [n_users, ld] output; ground truth as CSR aligned with its rows
