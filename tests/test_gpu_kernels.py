@@ -309,6 +309,55 @@ def test_rank_vs_oracle_bit_exact(ops, orc, F, I, C, K):
     assert np.array_equal(ops.mf_predict(dev(P), dev(Q), dev(u32), dev(i32)).cpu().numpy(), orc.mf_predict(P, Q, u32, i32))
 
 
+def _topk_scores(rng, count, K):
+    """score rows [9, count]: random; all equal; mixed +0.0 / -0.0 among +-1; four distinct values (long tie runs); a run of
+    the row's best score straddling every chunk boundary of topk_scores_kernel (the key buffer of 4 096, then 4 096 - K new
+    keys per chunk); ascending (every chunk replaces the running best); descending; the best score at both ends; a tie run at
+    the K-th place"""
+    S = rng.standard_normal((9, count)).astype(np.float32)
+    S[1] = 0.75
+    S[2] = rng.choice(np.array([-1.0, -0.0, 0.0, 1.0], np.float32), count)
+    S[3] = rng.integers(0, 4, count)
+    S[4] = -np.abs(S[4])
+    for c in range(4096, count, 4096 - K) if count > 4096 else range(min(64, count - 1), count, 64):
+        S[4, max(0, c - 40):c + 40] = 3.0
+    S[5] = np.sort(S[5])
+    S[6] = np.sort(S[6])[::-1]
+    S[7, 0] = S[7, -1] = S[7].max() + 1
+    srt = np.sort(S[8])[::-1]
+    hi, lo = srt[max(0, K - 1 - K // 4)], srt[min(count - 1, K + K // 4)]
+    S[8][(S[8] >= lo) & (S[8] <= hi)] = hi
+    return S
+
+
+@pytest.mark.parametrize("count", [1, 63, 64, 65, 4095, 4096, 4097, 8193, 26744])
+def test_topk_from_scores_vs_stable_sort(ops, count):
+    """drb_topk_from_scores (topk_scores_kernel: VAE, NeuMF and NFM scoring) bit for bit against a stable sort by score
+    descending, then position ascending (+0.0 == -0.0), with candidate ids (float32 out, ids in [2^16, 2^24)) and without (int64
+    positions), at K = 1, 50, 2 047 and 2 048 (K = count where count is smaller): one key buffer, and past it the chunks merged
+    with the running best K"""
+    rng = np.random.default_rng(count)
+    for K in sorted({min(count, k) for k in (1, 50, 2047, 2048)}):
+        S = _topk_scores(rng, count, K)
+        pos = np.argsort(-S, axis=1, kind="stable")[:, :K]
+        cands = rng.integers(1 << 16, 1 << 24, S.shape).astype(np.int64)
+        cands[:, -1] = (1 << 24) - 1                             # the largest id a float32 holds exactly
+        got_i = ops.topk_from_scores(dev(S), None, K).cpu().numpy()
+        assert got_i.dtype == np.int64 and np.array_equal(got_i, pos), (count, K)
+        got_f = ops.topk_from_scores(dev(S), dev(cands), K).cpu().numpy()
+        want_f = np.take_along_axis(cands, pos, 1).astype(np.float32)
+        assert got_f.dtype == np.float32 and np.array_equal(got_f, want_f), (count, K)
+
+
+def test_topk_from_scores_refuses_bad_k(ops):
+    from daisyrec_b200._lib import DrbError
+    S = dev(np.zeros((2, 5000), np.float32))
+    for K, cnt in ((2049, 5000), (11, 10)):
+        for cands in (None, dev(np.zeros((2, cnt), np.int64))):
+            with pytest.raises(DrbError, match="topk_from_scores: bad arguments"):
+                ops.topk_from_scores(S[:, :cnt].contiguous(), cands, K)
+
+
 # ------------------------------------------------------------------ the DataLoader's epoch order on the device
 @pytest.mark.parametrize("n", [1, 2, 3, 5, 623, 624, 625, 1000, 4097, 100_003, 3_000_000])
 def test_randperm_torch_is_bit_exact(n):
