@@ -150,6 +150,9 @@ static int ubucket_switch()
 // the phase (bucket sizes follow the user degrees); at least kUbMinUsers, at most what a 64 KB shared accumulator holds.  0 when
 // the mode cannot run the problem (more than kUbMaxBuckets buckets: the per-CTA histogram would not fit shared memory).
 constexpr int kUbMinUsers = 16, kUbMaxBuckets = 8192;
+// dynamic shared memory the staged SGD user side may take (two CTAs per SM keep fitting next to the 32 KB static index tiles):
+// 51 KB at F = 64 and 66 users per bucket (ML-20M on 132 SMs); it stages up to 84 users per bucket at F = 64, 167 at F = 32
+constexpr size_t kUbStagedSmem = 65536;
 constexpr long long kUbTimedBatch = 1 << 19;   // triples per step of the on-device timing problem (lean_autotune)
 static int ub_users_for(int U, int F, long long batch)
 {
@@ -163,17 +166,19 @@ static int ub_users_for(int U, int F, long long batch)
     return (nbk <= kUbMaxBuckets && batch + 4 * nbk < (1LL << 31)) ? ub : 0;
 }
 
-// The bucketed mode's scratch (counters, bucket ranges, partitioned triples): library-owned, grow-only, one per device and stream;
-// it depends on the batch, so it cannot live in the workspace.  Its counters are cleared before every launch.  Each buffer lives
-// as long as the process: about 16 B x the largest batch of bucketed steps launched on that stream (16.8 MB at B = 1 M), so a
+// The bucketed mode's scratch (counters, bucket ranges, user norm cache, partitioned triples): library-owned, grow-only, one per
+// device and stream; it depends on the batch, so it cannot live in the workspace.  Its counters are cleared before every launch,
+// the norm cache (staged SGD mode only) is filled by the launch itself.  Each buffer lives as long as the process: about
+// 16 B x the largest batch of bucketed steps launched on that stream + 8 B per user (17.9 MB at B = 1 M and ML-20M's users), so a
 // caller that trains on many streams holds one such buffer per stream.
-static int ub_scratch(StepParams &p, cudaStream_t st)
+static int ub_scratch(StepParams &p, cudaStream_t st, bool staged)
 {
     static std::mutex mu;
     static std::map<std::pair<int, cudaStream_t>, std::pair<void *, size_t>> bufs;
     const size_t nbk = (size_t)p.ub_buckets;
     const size_t cnt_b = align256(sizeof(unsigned) * (2 * nbk + 1)), rng_b = align256(sizeof(int) * 2 * nbk);
-    const size_t need = cnt_b + rng_b + sizeof(int4) * (size_t)p.batch;
+    const size_t nrm_b = staged ? align256(sizeof(float2) * (size_t)p.U) : 0;
+    const size_t need = cnt_b + rng_b + nrm_b + sizeof(int4) * (size_t)p.batch;
     int dev = 0;
     DRB_CUDA(cudaGetDevice(&dev));
     std::lock_guard<std::mutex> lock(mu);
@@ -190,7 +195,8 @@ static int ub_scratch(StepParams &p, cudaStream_t st)
     char *b = (char *)e.first;
     p.ub_count = (unsigned *)b;
     p.ub_range = (int *)(b + cnt_b);
-    p.ub_t = (int4 *)(b + cnt_b + rng_b);
+    p.ub_norm = staged ? (float2 *)(b + cnt_b + rng_b) : nullptr;
+    p.ub_t = (int4 *)(b + cnt_b + rng_b + nrm_b);
     DRB_CUDA(cudaMemsetAsync(p.ub_count, 0, sizeof(unsigned) * (2 * nbk + 1), st));
     return DRB_OK;
 }
@@ -220,10 +226,14 @@ static int launch_kernel(StepKernel k, StepParams &p, cudaStream_t st, bool keep
         p.ub_users = ub_users_for(p.U, p.F, p.batch);
         DRB_REQUIRE(p.ub_users > 0, "user-bucketed step: %d users in more than %d buckets", p.U, kUbMaxBuckets);
         p.ub_buckets = (p.U + p.ub_users - 1) / p.ub_users;
+        // SGD stages the bucket's user rows (two slots: the current bucket's and the prefetched next one's) next to the
+        // accumulator, when both fit kUbStagedSmem; wider buckets keep the accumulate-then-sweep user side
         const size_t acc = sizeof(float) * (size_t)p.ub_users * (p.F + 1) + sizeof(unsigned) * p.ub_users;
-        const size_t hist = 2 * sizeof(unsigned) * (size_t)p.ub_buckets;
-        smem = ((acc > hist ? acc : hist) + 15) / 16 * 16;
-        const int rc = ub_scratch(p, st);
+        const size_t rows = 2 * sizeof(float) * (size_t)p.ub_users * p.F;
+        const bool staged = p.opt == DRB_OPT_SGD && acc + rows <= kUbStagedSmem;
+        const size_t need = acc + (staged ? rows : 0), hist = 2 * sizeof(unsigned) * (size_t)p.ub_buckets;
+        smem = ((need > hist ? need : hist) + 15) / 16 * 16;
+        const int rc = ub_scratch(p, st, staged);
         if (rc != DRB_OK) return rc;
     }
     // occupancy of the chosen instantiation, cached per device (the query costs microseconds and this runs once per step in the

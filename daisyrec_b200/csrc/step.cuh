@@ -116,7 +116,10 @@ struct StepParams {
     unsigned *ub_count = nullptr;  // [2 * ub_buckets + 1]: triples per bucket, reservation cursors, work counter; zero between steps
     int *ub_range = nullptr;       // [2 * ub_buckets]: first and end position of bucket b in the partitioned triples
     int4 *ub_t = nullptr;          // [batch]: the partitioned triples as (u, i, j, 0) records, bucket after bucket
-    void *ub_spare[2] = {};        // unused: keeps the size, so the parameters after StepParams (p2p.cu) keep their offsets
+    // [U]: (||p_u||^2, ||p_u||_1) of every user row.  Set (SGD only) when the bucket's user rows are staged in shared memory
+    // and updated as the bucket completes; nullptr: the user gradients go to gP / cntU and phase 2 applies them
+    float2 *ub_norm = nullptr;
+    void *ub_spare = nullptr;      // unused: keeps the size, so the parameters after StepParams (p2p.cu) keep their offsets
 };
 
 // One step on a batch of B triples (bu, bi, bj) of a U x I problem with F factors, with the hyper-parameters of h; the

@@ -54,6 +54,31 @@ struct AdamCoef {
     float step_size, bc2_sqrt;
 };
 
+// Gradient of one element of a touched row: its accumulated part g plus the regulariser, count x f(theta), for the row's two
+// roles (ca / cb occurrences, ia / ib the inverse batch norms; user rows: cb = 0).  The dense sweep and the bucketed SGD user
+// update (bpr_steps_body) both take it from here, so they compile the same fp32 expression.
+__device__ __forceinline__ float reg_grad(float x, float g, float ca, float ia, float cb, float ib, const StepParams &p)
+{
+    const float sg = p.reg1 * sgnf(x);
+    return g + (ca * (sg + p.reg2 * x * ia) + cb * (sg + p.reg2 * x * ib));
+}
+
+// ||row||^2 and ||row||_1 of a user row of CH 4-float chunks, one chunk per lane: the CH lanes of a row are consecutive and CH
+// divides 32, so xor-shuffles within them finish both sums (every lane of the warp must take part)
+template <int CH>
+__device__ __forceinline__ float2 row_norms(float4 v)
+{
+    float s2 = 0.f, l1 = 0.f;
+    s2 = fmaf(v.x, v.x, s2); s2 = fmaf(v.y, v.y, s2); s2 = fmaf(v.z, v.z, s2); s2 = fmaf(v.w, v.w, s2);
+    l1 = fabsf(v.x) + fabsf(v.y) + fabsf(v.z) + fabsf(v.w);
+#pragma unroll
+    for (int off = 1; off < CH; off <<= 1) {
+        s2 += __shfl_xor_sync(0xffffffffu, s2, off);
+        l1 += __shfl_xor_sync(0xffffffffu, l1, off);
+    }
+    return make_float2(s2, l1);
+}
+
 // Apply the accumulated gradient of ONE table row (all W lanes of the group cooperate).
 // cnt_a / cnt_b: occurrences weighted by inv_a / inv_b (user rows: cnt_b = 0).
 template <int VEC, int W, int NCH, int OPT>
@@ -117,15 +142,19 @@ __device__ __forceinline__ void apply_row(float *theta_row, float *g_row, float 
 // DET (deterministic mode): the gradient is read from the fixed-point sums and assembled with the regulariser in fp64, rounded
 // to fp32 once, and the SGD step rounds lr * g before the subtraction -- the fp64-accumulating oracle's arithmetic, so that the
 // result does not depend on how the compiler contracts the fp32 expression.
-template <int VEC, int W, int NCH, int OPT, bool USERS_ONLY = false, bool DET = false>
+// USERS_ONLY: the user rows alone (peer exchange: item rows have an owner rank); ITEMS_ONLY: the item rows alone (the bucketed
+// SGD step has updated every touched user row in phase 1).
+template <int VEC, int W, int NCH, int OPT, bool USERS_ONLY = false, bool DET = false, bool ITEMS_ONLY = false>
 __device__ __forceinline__ void dense_sweep(const StepParams &p, const Norms &nm, const AdamCoef &ac, int gl, int group,
                                             int groups_per_cta, int chunks)
 {
+    static_assert(!(USERS_ONLY && ITEMS_ONLY), "one half or both");
     constexpr int R = (OPT == DRB_OPT_SGD) ? ((NCH * VEC <= 4) ? 4 : 2) : ((NCH * VEC <= 4) ? 2 : 1);
-    const long long rows = USERS_ONLY ? (long long)p.U : (long long)p.U + p.I;   // peer exchange: item rows have an owner rank
+    const long long rows = USERS_ONLY ? (long long)p.U : (long long)p.U + p.I;
+    const long long first = ITEMS_ONLY ? (long long)p.U : 0;
     const long long tg = (long long)gridDim.x * groups_per_cta;
     const int F = p.F;
-    for (long long r0 = (long long)blockIdx.x * groups_per_cta + group; r0 < rows; r0 += tg * R) {
+    for (long long r0 = first + (long long)blockIdx.x * groups_per_cta + group; r0 < rows; r0 += tg * R) {
         float *th_p[R], *g_p[R], *m_p[R], *v_p[R];
         long long *g64_p[R];
         unsigned long long cnt[R];
@@ -135,7 +164,7 @@ __device__ __forceinline__ void dense_sweep(const StepParams &p, const Norms &nm
         for (int k = 0; k < R; ++k) {
             long long r = r0 + (long long)k * tg;
             act[k] = r < rows;
-            is_user[k] = r < p.U;
+            is_user[k] = !ITEMS_ONLY && r < p.U;
             long long it = is_user[k] ? r : r - p.U;
             size_t o = (size_t)(act[k] ? it : 0) * F;
             th_p[k] = (is_user[k] ? p.P : p.Q) + o;
@@ -181,10 +210,7 @@ __device__ __forceinline__ void dense_sweep(const StepParams &p, const Norms &nm
                         gg = (float)gd;
                     } else {
                         gg = p.gscale * g[k].c[ch].v[e];
-                        if (touched) {
-                            float sg = p.reg1 * sgnf(x);
-                            gg += ca * (sg + p.reg2 * x * ia) + cb * (sg + p.reg2 * x * ib);
-                        }
+                        if (touched) gg = reg_grad(x, gg, ca, ia, cb, ib, p);
                     }
                     if constexpr (OPT == DRB_OPT_SGD) {
                         t.v[e] = DET ? __fsub_rn(x, __fmul_rn(p.lr, gg)) : x - p.lr * gg;
@@ -270,6 +296,12 @@ struct NoExchange {
 // gradient rows and counts of the bucket in shared memory and write each touched gP row and cntU entry once with plain stores,
 // instead of one RED per occurrence into the (L2-missing) user accumulators.  Item side, loss and norms are unchanged; only the
 // fp32 summation order of the user gradient differs (the REDs leave it unspecified as well).
+// UBK under SGD, when the launcher provides the norm cache p.ub_norm (the staged rows fit shared memory): a claimed bucket's user
+// rows are bulk-copied into shared memory with its first tile and read from there, and each touched row takes its SGD update when
+// the bucket completes: every triple of user u is in u's bucket, so no other CTA reads p_u in the step.  The user norms that update
+// needs are known before phase 1: the cache holds ||p_u||^2 and ||p_u||_1 of every user row (filled once per launch, rewritten
+// by each update; an untouched row does not move under SGD), and the partition's histogram pass sums it over the batch.  gP and
+// cntU are never written, and phase 2 sweeps the item rows alone.
 template <int VEC, int W, int NCH, bool GEN, class XCH, bool LEAN = false, bool UBK = false>
 __device__ __forceinline__ void bpr_steps_body(StepParams &p, XCH &xch)
 {
@@ -284,7 +316,7 @@ __device__ __forceinline__ void bpr_steps_body(StepParams &p, XCH &xch)
     __shared__ __align__(128) int32_t s_idx[2][UBK ? 4 : 3][kTileMax];
     __shared__ uint64_t s_bar[2];
     __shared__ double s_red[8][kThreads / 32];
-    extern __shared__ __align__(16) unsigned char s_dyn[];   // UBK: partition histogram, then the bucket accumulator
+    extern __shared__ __align__(16) unsigned char s_dyn[];   // UBK: partition histogram, then (staged rows +) bucket accumulator
     __shared__ int s_claim[3];                               // UBK: claimed bucket, its first and end position
     __shared__ unsigned s_wsum[kThreads / 32];               // UBK: per-warp sums of the bucket-count scan
 
@@ -336,8 +368,9 @@ __device__ __forceinline__ void bpr_steps_body(StepParams &p, XCH &xch)
         mbar_expect_tx(&s_bar[b], bytes);
         tma_load_1d(&s_idx[b][0][0], p.ub_t + t0, bytes, &s_bar[b]);
     };
-    // UBK, thread 0: claim the next non-empty bucket through the work counter, publish it in s_claim and stage its first tile
-    auto claim = [&](int b) {
+    // UBK, thread 0: claim the next non-empty bucket through the work counter, publish it in s_claim and stage its first tile;
+    // dst != nullptr: its user rows join the same copy, into dst (row stride F)
+    auto claim = [&](int b, float *dst) {
         int k, c0 = 0, c1 = 0;
         do {
             k = (int)atomicAdd(p.ub_count + 2 * p.ub_buckets, 1u);
@@ -345,10 +378,34 @@ __device__ __forceinline__ void bpr_steps_body(StepParams &p, XCH &xch)
         } while (k < p.ub_buckets && c0 == c1);
         s_claim[0] = k; s_claim[1] = c0; s_claim[2] = c1;
         if (k < p.ub_buckets) {
-            asm volatile("fence.proxy.async.global;" ::: "memory");   // generic-proxy writes of the planes -> bulk copy
-            stage_ub(c0, min(c1 - c0, kTileMax), b);
+            asm volatile("fence.proxy.async.global;" ::: "memory");   // generic-proxy writes of the planes / rows -> bulk copy
+            if (dst == nullptr) {
+                stage_ub(c0, min(c1 - c0, kTileMax), b);
+            } else {
+                asm volatile("fence.proxy.async.shared::cta;" ::: "memory");   // the slot's generic reads before its refill
+                const int u0k = k * p.ub_users;
+                const uint32_t rb = (uint32_t)min(p.ub_users, p.U - u0k) * (uint32_t)F * 4u, tb = (uint32_t)min(c1 - c0, kTileMax) * 16u;
+                mbar_expect_tx(&s_bar[b], tb + rb);
+                tma_load_1d(&s_idx[b][0][0], p.ub_t + c0, tb, &s_bar[b]);
+                tma_load_1d(dst, p.P + (size_t)u0k * F, rb, &s_bar[b]);
+            }
         }
     };
+    // UBK + SGD with the norm cache: user rows staged and updated per bucket (see above); unorm: the cache is kept (regulariser on)
+    const bool ustage = UBK && p.ub_norm != nullptr;
+    const bool unorm = ustage && ((p.reg1 != 0.f) || (p.reg2 != 0.f));
+    if constexpr (UBK) {
+        if (unorm) {   // fill the norm cache: one pass over P per launch
+            const long long nt = (long long)p.U * (W * NCH);
+            for (long long k0 = (long long)blockIdx.x * kThreads; k0 < nt; k0 += (long long)gridDim.x * kThreads) {
+                const long long k = k0 + tid;
+                const float4 v = k < nt ? __ldcg(reinterpret_cast<const float4 *>(p.P) + k) : make_float4(0.f, 0.f, 0.f, 0.f);
+                const float2 n = row_norms<W * NCH>(v);
+                if (k < nt && k % (W * NCH) == 0) p.ub_norm[k / (W * NCH)] = n;
+            }
+            grid_barrier(&hdr->barrier, epoch);
+        }
+    }
 
     for (long long s = 0; s < p.n_steps; ++s) {
         const long long step = p.first_step + s;
@@ -371,6 +428,9 @@ __device__ __forceinline__ void bpr_steps_body(StepParams &p, XCH &xch)
         int bk = 0, r0 = 0, r1 = 0, tt = 0, u0 = 0, rows = 0;
         float *s_gp = nullptr;
         unsigned *s_cu = nullptr;
+        float *s_rows = nullptr, *s_pu = nullptr;   // ustage: both row slots, the current bucket's slot
+        int slot = 0;
+        float inv_u = 0.f;
         if constexpr (UBK) {
             const int NBK = p.ub_buckets, UBU = p.ub_users, RS = F + 1;
             unsigned *ucnt = p.ub_count, *ucur = p.ub_count + NBK;
@@ -379,10 +439,32 @@ __device__ __forceinline__ void bpr_steps_body(StepParams &p, XCH &xch)
             for (int b = tid; b < NBK; b += kThreads) s_hist[b] = 0u;
             __syncthreads();
             const long long g0 = (long long)blockIdx.x * kThreads + tid, gstride = (long long)gridDim.x * kThreads;
-            for (long long t = g0; t < nb; t += gstride) atomicAdd(&s_hist[__ldg(p.bu + base + t) / UBU], 1u);
+            float h_s2 = 0.f, h_l1 = 0.f;   // unorm: this thread's share of the batch's user norms, from the norm cache
+            for (long long t = g0; t < nb; t += gstride) {
+                const int u = __ldg(p.bu + base + t);
+                atomicAdd(&s_hist[u / UBU], 1u);
+                if (unorm) {
+                    const float2 n = __ldcg(p.ub_norm + u);
+                    h_s2 += n.x;
+                    h_l1 += n.y;
+                }
+            }
+            if (unorm) {
+#pragma unroll
+                for (int off = 16; off >= 1; off >>= 1) {
+                    h_s2 += __shfl_xor_sync(0xffffffffu, h_s2, off);
+                    h_l1 += __shfl_xor_sync(0xffffffffu, h_l1, off);
+                }
+                if (lane == 0) { s_red[4][warp] = (double)h_s2; s_red[1][warp] = (double)h_l1; }
+            }
             __syncthreads();
             for (int b = tid; b < NBK; b += kThreads)
                 if (s_hist[b] != 0u) red_add_u32(ucnt + b, s_hist[b]);
+            if (unorm && (tid == 1 || tid == 4)) {   // l1u, s2u: one fp64 atomic per CTA; final after the next grid barrier
+                double v = 0.0;
+                for (int w = 0; w < kThreads / 32; ++w) { v += s_red[tid][w]; s_red[tid][w] = 0.0; }
+                if (v != 0.0) atomicAdd(&acc[tid], v);
+            }
             grid_barrier(&hdr->barrier, epoch);
             // exclusive scan of the counts in every CTA; CTA 0 publishes the ranges; each CTA reserves its slice of every bucket
             // it holds triples of
@@ -418,10 +500,16 @@ __device__ __forceinline__ void bpr_steps_body(StepParams &p, XCH &xch)
             asm volatile("fence.proxy.async.global;" ::: "memory");   // the records are read back by bulk copies (async proxy)
             grid_barrier(&hdr->barrier, epoch);
             for (long long k = g0; k < 2LL * NBK; k += gstride) ucnt[k] = 0u;   // counts, cursors: zero for the next step
-            s_gp = reinterpret_cast<float *>(s_dyn);
+            // ustage: two slots of UBU staged user rows (the current bucket's and the next one's) before the accumulator
+            s_rows = reinterpret_cast<float *>(s_dyn);
+            s_gp = s_rows + (ustage ? 2 * UBU * F : 0);
             s_cu = reinterpret_cast<unsigned *>(s_gp + UBU * RS);
+            if (unorm) {
+                const double nu = sqrt(((const volatile double *)acc)[4]);   // as phase 2 derives it
+                inv_u = nu > 0 ? (float)(1.0 / nu) : 0.f;
+            }
             // ---- phase 1 over whole buckets, claimed dynamically (bucket sizes follow the user degrees)
-            if (tid == 0) claim(0);
+            if (tid == 0) claim(0, ustage ? s_rows : nullptr);
             __syncthreads();
             bk = s_claim[0]; r0 = s_claim[1]; r1 = s_claim[2]; tt = r0;
         } else {
@@ -432,13 +520,14 @@ __device__ __forceinline__ void bpr_steps_body(StepParams &p, XCH &xch)
                 if (tt == r0) {                                  // first tile of a bucket: zero its accumulator rows
                     u0 = bk * p.ub_users;
                     rows = min(p.ub_users, p.U - u0);
+                    s_pu = s_rows + slot * p.ub_users * F;
                     for (int k = tid; k < rows * (F + 1); k += kThreads) s_gp[k] = 0.f;
                     for (int k = tid; k < rows; k += kThreads) s_cu[k] = 0u;
                     __syncthreads();                             // zeroed; every thread has read s_claim
                 }
                 if (tid == 0) {                                  // prefetch: the bucket's next tile or the next bucket
                     if (tt + kTileMax < r1) stage_ub(tt + kTileMax, min(r1 - tt - kTileMax, kTileMax), buf ^ 1);
-                    else claim(buf ^ 1);
+                    else claim(buf ^ 1, ustage ? s_rows + (slot ^ 1) * p.ub_users * F : nullptr);
                 }
             } else {
                 long long t_n = t_i + gridDim.x;
@@ -477,7 +566,21 @@ __device__ __forceinline__ void bpr_steps_body(StepParams &p, XCH &xch)
                     ou[r] = (RowOff)iu[r] * (RowOff)F;
                     oi[r] = (RowOff)ii[r] * (RowOff)F;
                     oj[r] = (RowOff)ij[r] * (RowOff)F;
-                    rp[r] = load_row<VEC, W, NCH>(p.P + ou[r], gl, chunks, ok[r]);
+                    bool staged = false;
+                    if constexpr (UBK) {
+                        if (ustage) {                        // the bucket's staged row (a quarter-warp reads one 128-byte segment)
+                            staged = true;
+                            const float *sr = s_pu + (ok[r] ? iu[r] - u0 : 0) * F;
+#pragma unroll
+                            for (int ch = 0; ch < NCH; ++ch) {
+                                const int c = gl + ch * W;
+                                float4 t = make_float4(0.f, 0.f, 0.f, 0.f);
+                                if (ok[r] && c < chunks) t = *reinterpret_cast<const float4 *>(sr + c * VEC);
+                                rp[r].c[ch].v[0] = t.x; rp[r].c[ch].v[1] = t.y; rp[r].c[ch].v[2] = t.z; rp[r].c[ch].v[3] = t.w;
+                            }
+                        }
+                    }
+                    if (!staged) rp[r] = load_row<VEC, W, NCH>(p.P + ou[r], gl, chunks, ok[r]);
                     rqi[r] = load_row<VEC, W, NCH>(p.Q + oi[r], gl, chunks, ok[r]);
                     rqj[r] = load_row<VEC, W, NCH>(p.Q + oj[r], gl, chunks, ok[r] && !pw);
                 }
@@ -575,8 +678,9 @@ __device__ __forceinline__ void bpr_steps_body(StepParams &p, XCH &xch)
                                 l1i += fabsf(b); s2i = fmaf(b, b, s2i);
                                 l1j += fabsf(d); s2j = fmaf(d, d, s2j);
                             }
-                        t_l1u += l1u; t_l1i += l1i; t_l1j += l1j;
-                        t_s2u += s2u; t_s2i += s2i; t_s2j += s2j;
+                        if (!unorm) { t_l1u += l1u; t_s2u += s2u; }   // unorm: the partition has summed the user norms
+                        t_l1i += l1i; t_l1j += l1j;
+                        t_s2i += s2i; t_s2j += s2j;
                     }
                     if (p.apply) {
 #pragma unroll
@@ -649,7 +753,33 @@ __device__ __forceinline__ void bpr_steps_body(StepParams &p, XCH &xch)
             buf ^= 1;
             if constexpr (UBK) {
                 tt += kTileMax;
-                if (tt >= r1) {   // the bucket is complete: one plain store per touched row and counter; untouched rows keep zeros
+                if (tt >= r1 && ustage) {
+                    // the bucket is complete: each touched row takes its SGD update from the staged row and is stored back, with
+                    // its new norms (one chunk per thread, the W * NCH chunks of a row on consecutive lanes); untouched rows stay
+                    constexpr int CH = W * NCH;
+                    const int n = rows * CH;
+                    for (int k0 = 0; k0 < n; k0 += kThreads) {
+                        const int k = k0 + tid, r = k / CH, c = k - r * CH;
+                        const bool live = k < n && s_cu[r] != 0u;
+                        float4 th = make_float4(0.f, 0.f, 0.f, 0.f);
+                        if (live) {
+                            const float *a = s_pu + r * F + c * VEC, *g = s_gp + r * (F + 1) + c * VEC;
+                            const float cnt = (float)s_cu[r];
+                            th.x = a[0] - p.lr * reg_grad(a[0], p.gscale * g[0], cnt, inv_u, 0.f, 0.f, p);
+                            th.y = a[1] - p.lr * reg_grad(a[1], p.gscale * g[1], cnt, inv_u, 0.f, 0.f, p);
+                            th.z = a[2] - p.lr * reg_grad(a[2], p.gscale * g[2], cnt, inv_u, 0.f, 0.f, p);
+                            th.w = a[3] - p.lr * reg_grad(a[3], p.gscale * g[3], cnt, inv_u, 0.f, 0.f, p);
+                            __stcg(reinterpret_cast<float4 *>(p.P + (size_t)(u0 + r) * F + c * VEC), th);
+                        }
+                        if (unorm) {
+                            const float2 nrm = row_norms<CH>(th);
+                            if (live && c == 0) __stcg(p.ub_norm + u0 + r, nrm);
+                        }
+                    }
+                    __syncthreads();   // slot and accumulator free; s_claim holds the bucket claimed during this tile
+                    bk = s_claim[0]; r0 = s_claim[1]; r1 = s_claim[2]; tt = r0;
+                    slot ^= 1;
+                } else if (tt >= r1) {   // the bucket is complete: one plain store per touched row and counter; untouched rows keep zeros
                     for (int k = tid; k < rows * chunks; k += kThreads) {
                         const int r = k / chunks, c = k - r * chunks;
                         if (s_cu[r] == 0u) continue;
@@ -749,7 +879,9 @@ __device__ __forceinline__ void bpr_steps_body(StepParams &p, XCH &xch)
                         dense_sweep<VEC, W, NCH, DRB_OPT_RMSPROP, false, true>(p, nm, ac, gl, group, GROUPS, chunks);
                 }
             } else if (dense || p.opt != DRB_OPT_SGD) {   // stateful optimisers always sweep (claim mode is SGD only)
-                if (p.opt == DRB_OPT_SGD)
+                if (ustage)                        // the user rows took their update when their bucket completed
+                    dense_sweep<VEC, W, NCH, DRB_OPT_SGD, false, false, UBK>(p, nm, ac, gl, group, GROUPS, chunks);
+                else if (p.opt == DRB_OPT_SGD)
                     dense_sweep<VEC, W, NCH, DRB_OPT_SGD, XCH::kActive>(p, nm, ac, gl, group, GROUPS, chunks);
                 else if (p.opt == DRB_OPT_ADAM)
                     dense_sweep<VEC, W, NCH, DRB_OPT_ADAM, XCH::kActive>(p, nm, ac, gl, group, GROUPS, chunks);
