@@ -137,6 +137,14 @@ static StepKernel pick_lean_ub(int W, int NCH)
     if (NCH == 2) return mf_bpr_steps_lean_kernel<4, 8, 2, true>;
     return nullptr;
 }
+// its staged SGD form (user rows staged per bucket, tiles sorted by user, item regulariser per occurrence): its own
+// instantiation, so that neither form carries the other's registers; launch_kernel swaps it in when the launch can stage
+static StepKernel staged_twin(StepKernel k)
+{
+    if (k == mf_bpr_steps_lean_kernel<4, 8, 1, true>) return mf_bpr_steps_lean_kernel<4, 8, 1, true, true>;
+    if (k == mf_bpr_steps_lean_kernel<4, 8, 2, true>) return mf_bpr_steps_lean_kernel<4, 8, 2, true, true>;
+    return nullptr;
+}
 static int ubucket_switch()
 {
     static const int v = [] {
@@ -147,11 +155,13 @@ static int ubucket_switch()
 }
 
 // Users per bucket of the user-bucketed mode: about 8 buckets per resident CTA, so that the dynamic claiming of buckets balances
-// the phase (bucket sizes follow the user degrees); at least kUbMinUsers, at most what a 64 KB shared accumulator holds.  0 when
-// the mode cannot run the problem (more than kUbMaxBuckets buckets: the per-CTA histogram would not fit shared memory).
+// the phase (bucket sizes follow the user degrees); at least kUbMinUsers, at most what a 64 KB shared accumulator holds and
+// kUbMaxRows (the keys of the per-tile user sort).  0 when the mode cannot run the problem (more than kUbMaxBuckets buckets: the
+// per-CTA histogram would not fit shared memory).
 constexpr int kUbMinUsers = 16, kUbMaxBuckets = 8192;
-// dynamic shared memory the staged SGD user side may take (two CTAs per SM keep fitting next to the 32 KB static index tiles):
-// 51 KB at F = 64 and 66 users per bucket (ML-20M on 132 SMs); it stages up to 84 users per bucket at F = 64, 167 at F = 32
+// dynamic shared memory the staged SGD user side may take (two CTAs per SM keep fitting next to the 39 KB of static index tiles
+// and per-tile sort arrays): 51 KB at F = 64 and 66 users per bucket (ML-20M on 132 SMs); it stages up to 84 users per bucket at
+// F = 64, 168 at F = 32
 constexpr size_t kUbStagedSmem = 65536;
 constexpr long long kUbTimedBatch = 1 << 19;   // triples per step of the on-device timing problem (lean_autotune)
 static int ub_users_for(int U, int F, long long batch)
@@ -159,17 +169,18 @@ static int ub_users_for(int U, int F, long long batch)
     const int target = 8 * DRB_MINB * sm_count();
     int ub = (U + target - 1) / target;
     if (ub < kUbMinUsers) ub = kUbMinUsers;
-    const int cap = 65536 / ((F + 1) * 4 + 4);
+    const int cap = 65536 / ((F + 1) * 4 + 4);   // width rule: F + 1 floats and a counter per user (the accumulator takes F)
     if (ub > cap) ub = cap;
+    if (ub > kUbMaxRows) ub = kUbMaxRows;
     if (ub < 1) return 0;
     const long long nbk = ((long long)U + ub - 1) / ub;
     return (nbk <= kUbMaxBuckets && batch + 4 * nbk < (1LL << 31)) ? ub : 0;
 }
 
-// The bucketed mode's scratch (counters, bucket ranges, user norm cache, partitioned triples): library-owned, grow-only, one per
-// device and stream; it depends on the batch, so it cannot live in the workspace.  Its counters are cleared before every launch,
-// the norm cache (staged SGD mode only) is filled by the launch itself.  Each buffer lives as long as the process: about
-// 16 B x the largest batch of bucketed steps launched on that stream + 8 B per user (17.9 MB at B = 1 M and ML-20M's users), so a
+// The bucketed mode's scratch (counters, bucket ranges, user and item norm cache, partitioned triples): library-owned, grow-only,
+// one per device and stream; it depends on the batch, so it cannot live in the workspace.  Its counters are cleared before every
+// launch, the norm cache (staged SGD mode only) is filled by the launch itself.  Each buffer lives as long as the process: about
+// 16 B x the largest batch of bucketed steps launched on that stream + 8 B per user and item (18.1 MB at B = 1 M and ML-20M), so a
 // caller that trains on many streams holds one such buffer per stream.
 static int ub_scratch(StepParams &p, cudaStream_t st, bool staged)
 {
@@ -177,7 +188,7 @@ static int ub_scratch(StepParams &p, cudaStream_t st, bool staged)
     static std::map<std::pair<int, cudaStream_t>, std::pair<void *, size_t>> bufs;
     const size_t nbk = (size_t)p.ub_buckets;
     const size_t cnt_b = align256(sizeof(unsigned) * (2 * nbk + 1)), rng_b = align256(sizeof(int) * 2 * nbk);
-    const size_t nrm_b = staged ? align256(sizeof(float2) * (size_t)p.U) : 0;
+    const size_t nrm_b = staged ? align256(sizeof(float2) * ((size_t)p.U + p.I)) : 0;
     const size_t need = cnt_b + rng_b + nrm_b + sizeof(int4) * (size_t)p.batch;
     int dev = 0;
     DRB_CUDA(cudaGetDevice(&dev));
@@ -228,13 +239,18 @@ static int launch_kernel(StepKernel k, StepParams &p, cudaStream_t st, bool keep
         p.ub_buckets = (p.U + p.ub_users - 1) / p.ub_users;
         // SGD stages the bucket's user rows (two slots: the current bucket's and the prefetched next one's) next to the
         // accumulator, when both fit kUbStagedSmem; wider buckets keep the accumulate-then-sweep user side
-        const size_t acc = sizeof(float) * (size_t)p.ub_users * (p.F + 1) + sizeof(unsigned) * p.ub_users;
+        // (accumulator row stride: F staged, F + 1 otherwise; the staged form adds the item regulariser once per occurrence in
+        // phase 1: unscaled gradients, one count per occurrence)
+        const size_t acc = sizeof(float) * (size_t)p.ub_users * p.F + sizeof(unsigned) * p.ub_users;
         const size_t rows = 2 * sizeof(float) * (size_t)p.ub_users * p.F;
-        const bool staged = p.opt == DRB_OPT_SGD && acc + rows <= kUbStagedSmem;
-        const size_t need = acc + (staged ? rows : 0), hist = 2 * sizeof(unsigned) * (size_t)p.ub_buckets;
+        const bool staged = p.opt == DRB_OPT_SGD && p.gscale == 1.f && p.neg_mult == 1.f && acc + rows <= kUbStagedSmem;
+        const size_t need = staged ? acc + rows : acc + sizeof(float) * (size_t)p.ub_users;
+        const size_t hist = 2 * sizeof(unsigned) * (size_t)p.ub_buckets;
         smem = ((need > hist ? need : hist) + 15) / 16 * 16;
         const int rc = ub_scratch(p, st, staged);
         if (rc != DRB_OK) return rc;
+        if (staged) k = staged_twin(k);
+        DRB_REQUIRE(k != nullptr, "user-bucketed step: no staged instantiation");
     }
     // occupancy of the chosen instantiation, cached per device (the query costs microseconds and this runs once per step in the
     // split multi-GPU / LightGCN / NeuMF paths); the dynamic shared-memory limit is a per-device function attribute

@@ -15,6 +15,7 @@ constexpr int kThreads = 256;
 constexpr int kTileMax = 1024;  // triples per staged index tile
 
 constexpr int kTileDefault = 512;
+constexpr int kUbMaxRows = 512;   // users per bucket of the user-bucketed mode at most (its per-tile sort keys)
 
 // Tile size for `per_cta` triples per CTA and step: the fewest equal tiles of at most `cap` triples (a multiple of 16), so every
 // CTA walks the same number of full tiles (cap 512: 3 543 per CTA -> 7 tiles of 512; cap 1 024 -> 4 tiles of 896).
@@ -61,6 +62,13 @@ __device__ __forceinline__ float reg_grad(float x, float g, float ca, float ia, 
 {
     const float sg = p.reg1 * sgnf(x);
     return g + (ca * (sg + p.reg2 * x * ia) + cb * (sg + p.reg2 * x * ib));
+}
+
+// The regulariser of reg_grad for ONE occurrence of a row (ia: the inverse batch norm of its role): the bucketed SGD step adds
+// it to each item gradient contribution in phase 1, the order in which autograd sums the reference's loss
+__device__ __forceinline__ float reg_term(float x, float ia, const StepParams &p)
+{
+    return p.reg1 * sgnf(x) + p.reg2 * x * ia;
 }
 
 // ||row||^2 and ||row||_1 of a user row of CH 4-float chunks, one chunk per lane: the CH lanes of a row are consecutive and CH
@@ -142,19 +150,16 @@ __device__ __forceinline__ void apply_row(float *theta_row, float *g_row, float 
 // DET (deterministic mode): the gradient is read from the fixed-point sums and assembled with the regulariser in fp64, rounded
 // to fp32 once, and the SGD step rounds lr * g before the subtraction -- the fp64-accumulating oracle's arithmetic, so that the
 // result does not depend on how the compiler contracts the fp32 expression.
-// USERS_ONLY: the user rows alone (peer exchange: item rows have an owner rank); ITEMS_ONLY: the item rows alone (the bucketed
-// SGD step has updated every touched user row in phase 1).
-template <int VEC, int W, int NCH, int OPT, bool USERS_ONLY = false, bool DET = false, bool ITEMS_ONLY = false>
+// USERS_ONLY: the user rows alone (peer exchange: item rows have an owner rank).
+template <int VEC, int W, int NCH, int OPT, bool USERS_ONLY = false, bool DET = false>
 __device__ __forceinline__ void dense_sweep(const StepParams &p, const Norms &nm, const AdamCoef &ac, int gl, int group,
                                             int groups_per_cta, int chunks)
 {
-    static_assert(!(USERS_ONLY && ITEMS_ONLY), "one half or both");
     constexpr int R = (OPT == DRB_OPT_SGD) ? ((NCH * VEC <= 4) ? 4 : 2) : ((NCH * VEC <= 4) ? 2 : 1);
     const long long rows = USERS_ONLY ? (long long)p.U : (long long)p.U + p.I;
-    const long long first = ITEMS_ONLY ? (long long)p.U : 0;
     const long long tg = (long long)gridDim.x * groups_per_cta;
     const int F = p.F;
-    for (long long r0 = first + (long long)blockIdx.x * groups_per_cta + group; r0 < rows; r0 += tg * R) {
+    for (long long r0 = (long long)blockIdx.x * groups_per_cta + group; r0 < rows; r0 += tg * R) {
         float *th_p[R], *g_p[R], *m_p[R], *v_p[R];
         long long *g64_p[R];
         unsigned long long cnt[R];
@@ -164,7 +169,7 @@ __device__ __forceinline__ void dense_sweep(const StepParams &p, const Norms &nm
         for (int k = 0; k < R; ++k) {
             long long r = r0 + (long long)k * tg;
             act[k] = r < rows;
-            is_user[k] = !ITEMS_ONLY && r < p.U;
+            is_user[k] = r < p.U;
             long long it = is_user[k] ? r : r - p.U;
             size_t o = (size_t)(act[k] ? it : 0) * F;
             th_p[k] = (is_user[k] ? p.P : p.Q) + o;
@@ -292,19 +297,23 @@ struct NoExchange {
 // operands in the same order as the general body, with ~1/3 fewer instructions per triple.
 //
 // UBK (user-bucketed, lean single-GPU fused steps only): every step first partitions its triples by user bucket into scratch
-// records (histogram, grid barrier, scan + reservation, scatter, grid barrier); phase 1 then has CTAs claim whole buckets, sum the user
-// gradient rows and counts of the bucket in shared memory and write each touched gP row and cntU entry once with plain stores,
-// instead of one RED per occurrence into the (L2-missing) user accumulators.  Item side, loss and norms are unchanged; only the
-// fp32 summation order of the user gradient differs (the REDs leave it unspecified as well).
-// UBK under SGD, when the launcher provides the norm cache p.ub_norm (the staged rows fit shared memory): a claimed bucket's user
+// records (histogram, grid barrier, scan + reservation, scatter, grid barrier); phase 1 then has CTAs claim whole buckets, sort
+// each tile of the bucket by user, sum the user gradient of each run of a user in registers, add the run sums and the counts of
+// the bucket in shared memory and write each touched gP row and cntU entry once with plain stores, instead of one RED per
+// occurrence into the (L2-missing) user accumulators.  Item side, loss and norms are unchanged; only the fp32 summation order of
+// the user gradient differs (the REDs leave it unspecified as well).
+// UBK + STAGED (SGD, when the staged rows fit shared memory; the launcher then provides the norm cache p.ub_norm): a claimed bucket's user
 // rows are bulk-copied into shared memory with its first tile and read from there, and each touched row takes its SGD update when
 // the bucket completes: every triple of user u is in u's bucket, so no other CTA reads p_u in the step.  The user norms that update
 // needs are known before phase 1: the cache holds ||p_u||^2 and ||p_u||_1 of every user row (filled once per launch, rewritten
 // by each update; an untouched row does not move under SGD), and the partition's histogram pass sums it over the batch.  gP and
-// cntU are never written, and phase 2 sweeps the item rows alone.
-template <int VEC, int W, int NCH, bool GEN, class XCH, bool LEAN = false, bool UBK = false>
+// cntU are never written.  The cache also holds the item rows' norms, which the scatter pass sums over the batch's i and j, so
+// phase 1 adds each occurrence's item regulariser to its gQ contribution; cntI is never written either, and phase 2 is the
+// dense theta -= lr gQ over the item rows alone.
+template <int VEC, int W, int NCH, bool GEN, class XCH, bool LEAN = false, bool UBK = false, bool STAGED = false>
 __device__ __forceinline__ void bpr_steps_body(StepParams &p, XCH &xch)
 {
+    static_assert(!STAGED || UBK, "the staged form is a form of the user-bucketed mode");
     static_assert(!(GEN && LEAN), "the lean body is BPR only");
     static_assert(!UBK || (LEAN && VEC == 4 && !XCH::kActive), "the user-bucketed mode is a single-GPU lean mode");
     using RowOff = typename RowOffset<LEAN>::type;
@@ -319,6 +328,9 @@ __device__ __forceinline__ void bpr_steps_body(StepParams &p, XCH &xch)
     extern __shared__ __align__(16) unsigned char s_dyn[];   // UBK: partition histogram, then (staged rows +) bucket accumulator
     __shared__ int s_claim[3];                               // UBK: claimed bucket, its first and end position
     __shared__ unsigned s_wsum[kThreads / 32];               // UBK: per-warp sums of the bucket-count scan
+    __shared__ int s_ucnt[kUbMaxRows], s_uoff[kUbMaxRows + 1];   // UBK: a tile's records per local user, their sorted offsets
+    __shared__ uint16_t s_perm[kTileMax];                    // UBK: the tile's records in local-user order
+    __shared__ float s_inv[3];                               // UBK, unorm: the step's inverse batch norms (u, i, j)
 
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
     const int gl = lane % W, gw = lane / W;
@@ -332,6 +344,8 @@ __device__ __forceinline__ void bpr_steps_body(StepParams &p, XCH &xch)
         mbar_init(&s_bar[1], 1);
         fence_mbar_init();
     }
+    if constexpr (UBK)
+        for (int k = tid; k < kUbMaxRows; k += kThreads) s_ucnt[k] = 0;   // each tile's sort leaves it zero again
     __syncthreads();
     if (*(volatile int *)&hdr->status != 0) return;   // split mode: a previous step already raised NaN
     uint32_t par0 = 0, par1 = 0;
@@ -392,14 +406,15 @@ __device__ __forceinline__ void bpr_steps_body(StepParams &p, XCH &xch)
         }
     };
     // UBK + SGD with the norm cache: user rows staged and updated per bucket (see above); unorm: the cache is kept (regulariser on)
-    const bool ustage = UBK && p.ub_norm != nullptr;
+    constexpr bool ustage = UBK && STAGED;
     const bool unorm = ustage && ((p.reg1 != 0.f) || (p.reg2 != 0.f));
     if constexpr (UBK) {
-        if (unorm) {   // fill the norm cache: one pass over P per launch
-            const long long nt = (long long)p.U * (W * NCH);
+        if (unorm) {   // fill the norm cache: one pass over P and Q per launch (the item rows' entries follow the users')
+            const long long nu = (long long)p.U * (W * NCH), nt = nu + (long long)p.I * (W * NCH);
             for (long long k0 = (long long)blockIdx.x * kThreads; k0 < nt; k0 += (long long)gridDim.x * kThreads) {
                 const long long k = k0 + tid;
-                const float4 v = k < nt ? __ldcg(reinterpret_cast<const float4 *>(p.P) + k) : make_float4(0.f, 0.f, 0.f, 0.f);
+                const float4 *src = k < nu ? reinterpret_cast<const float4 *>(p.P) + k : reinterpret_cast<const float4 *>(p.Q) + (k - nu);
+                const float4 v = k < nt ? __ldcg(src) : make_float4(0.f, 0.f, 0.f, 0.f);
                 const float2 n = row_norms<W * NCH>(v);
                 if (k < nt && k % (W * NCH) == 0) p.ub_norm[k / (W * NCH)] = n;
             }
@@ -423,16 +438,16 @@ __device__ __forceinline__ void bpr_steps_body(StepParams &p, XCH &xch)
         int buf = 0;
         long long t_i = blockIdx.x;
         // UBK: claimed bucket bk, its triples [r0, r1) in the partitioned records, position tt of the current tile; the gradient
-        // rows and counts of its users u0 .. u0 + rows - 1 sum in s_gp / s_cu (row stride F + 1 against bank conflicts between
-        // the groups of a warp)
+        // rows and counts of its users u0 .. u0 + rows - 1 sum in s_gp / s_cu (row stride RS: F under ustage, 16-byte aligned
+        // rows for the run sums; F + 1 otherwise, against bank conflicts between the groups of a warp in the per-triple atomics)
         int bk = 0, r0 = 0, r1 = 0, tt = 0, u0 = 0, rows = 0;
+        const int RS = ustage ? F : F + 1;
         float *s_gp = nullptr;
         unsigned *s_cu = nullptr;
         float *s_rows = nullptr, *s_pu = nullptr;   // ustage: both row slots, the current bucket's slot
         int slot = 0;
-        float inv_u = 0.f;
         if constexpr (UBK) {
-            const int NBK = p.ub_buckets, UBU = p.ub_users, RS = F + 1;
+            const int NBK = p.ub_buckets, UBU = p.ub_users;
             unsigned *ucnt = p.ub_count, *ucur = p.ub_count + NBK;
             // ---- partition: per-CTA histogram of the bucket ids -> global counts
             unsigned *s_hist = reinterpret_cast<unsigned *>(s_dyn), *s_off = s_hist + NBK;
@@ -491,11 +506,32 @@ __device__ __forceinline__ void bpr_steps_body(StepParams &p, XCH &xch)
             __syncthreads();
             // ---- scatter this CTA's triples into the partitioned records (the same triples as the histogram pass); a CTA holds
             // about two triples per bucket, so these stores land at random: one 16-byte store per triple, not three 4-byte ones
+            // unorm: this pass also sums the item rows' cached norms over the batch (l1i, l1j, s2i, s2j)
+            float h_in[4] = {0.f, 0.f, 0.f, 0.f};
             for (long long t = g0; t < nb; t += gstride) {
                 const int u = __ldg(p.bu + base + t), b = u / UBU;
                 const int i = __ldg(p.bi + base + t), j = __ldg(p.bj + base + t);
                 const unsigned pos = s_off[b] + atomicAdd(&s_hist[b], 1u);
                 p.ub_t[pos] = make_int4(u, i, j, 0);
+                if (unorm) {
+                    const float2 ni = __ldcg(p.ub_norm + p.U + i), nj = __ldcg(p.ub_norm + p.U + j);
+                    h_in[0] += ni.y; h_in[1] += nj.y; h_in[2] += ni.x; h_in[3] += nj.x;
+                }
+            }
+            if (unorm) {
+#pragma unroll
+                for (int q = 0; q < 4; ++q) {
+                    float v = h_in[q];
+#pragma unroll
+                    for (int off = 16; off >= 1; off >>= 1) v += __shfl_xor_sync(0xffffffffu, v, off);
+                    if (lane == 0) s_red[q < 2 ? 2 + q : 3 + q][warp] = (double)v;
+                }
+                __syncthreads();
+                if (tid == 2 || tid == 3 || tid == 5 || tid == 6) {   // one fp64 atomic per CTA each; final after the barrier
+                    double v = 0.0;
+                    for (int w = 0; w < kThreads / 32; ++w) { v += s_red[tid][w]; s_red[tid][w] = 0.0; }
+                    if (v != 0.0) atomicAdd(&acc[tid], v);
+                }
             }
             asm volatile("fence.proxy.async.global;" ::: "memory");   // the records are read back by bulk copies (async proxy)
             grid_barrier(&hdr->barrier, epoch);
@@ -504,9 +540,9 @@ __device__ __forceinline__ void bpr_steps_body(StepParams &p, XCH &xch)
             s_rows = reinterpret_cast<float *>(s_dyn);
             s_gp = s_rows + (ustage ? 2 * UBU * F : 0);
             s_cu = reinterpret_cast<unsigned *>(s_gp + UBU * RS);
-            if (unorm) {
-                const double nu = sqrt(((const volatile double *)acc)[4]);   // as phase 2 derives it
-                inv_u = nu > 0 ? (float)(1.0 / nu) : 0.f;
+            if (ustage && tid < 3) {   // as phase 2 derives them; read from shared memory where used (fewer live registers)
+                const double n = unorm ? sqrt(((const volatile double *)acc)[tid + 4]) : 0.0;
+                s_inv[tid] = n > 0 ? (float)(1.0 / n) : 0.f;
             }
             // ---- phase 1 over whole buckets, claimed dynamically (bucket sizes follow the user degrees)
             if (tid == 0) claim(0, ustage ? s_rows : nullptr);
@@ -521,7 +557,7 @@ __device__ __forceinline__ void bpr_steps_body(StepParams &p, XCH &xch)
                     u0 = bk * p.ub_users;
                     rows = min(p.ub_users, p.U - u0);
                     s_pu = s_rows + slot * p.ub_users * F;
-                    for (int k = tid; k < rows * (F + 1); k += kThreads) s_gp[k] = 0.f;
+                    for (int k = tid; k < rows * RS; k += kThreads) s_gp[k] = 0.f;
                     for (int k = tid; k < rows; k += kThreads) s_cu[k] = 0u;
                     __syncthreads();                             // zeroed; every thread has read s_claim
                 }
@@ -539,8 +575,82 @@ __device__ __forceinline__ void bpr_steps_body(StepParams &p, XCH &xch)
             constexpr int XS = UBK ? 4 : 1;
             const int32_t *xu = s_idx[buf][0], *xi = UBK ? xu + 1 : s_idx[buf][1], *xj = UBK ? xu + 2 : s_idx[buf][2];
             float t_loss = 0.f, t_l1u = 0.f, t_l1i = 0.f, t_l1j = 0.f, t_s2u = 0.f, t_s2i = 0.f, t_s2j = 0.f, t_gb0 = 0.f;
+            // UBK + ustage: the tile's records are counting-sorted by local user into s_perm (user ul's run is
+            // s_perm[s_uoff[ul] .. s_uoff[ul + 1])), and group g walks the sorted positions [lo, hi) = [g span, (g + 1) span), UNR
+            // consecutive ones at a time.  It sums the user gradient of a run in registers (ua) and adds it to s_gp when the user
+            // changes: with a plain read-add-write when the whole run lies in [lo, hi) (no other group holds it in this tile), with
+            // shared-memory atomics when the run crosses a slice boundary (at most the first and the last run of a slice).  The
+            // histogram is the tile's share of s_cu.  Without ustage (Adam, buckets too wide to stage: about one triple per user
+            // and tile at the widths these run, where the sort costs more than it saves) the records are walked as in the plain
+            // body, and each triple's user gradient and count are added with shared-memory atomics (row stride F + 1).
+            int lo = 0, hi = 0, span = 0, urun = -1;
+            constexpr bool sorted = UBK && STAGED;
+            Vec<VEC> ua[NCH];
+            if constexpr (UBK) {
+                constexpr int PT = kTileMax / kThreads;   // records per thread
+                if (sorted) {
+                    int key[PT], rank[PT];
+#pragma unroll
+                    for (int q = 0; q < PT; ++q) {
+                        const int k = tid + q * kThreads;
+                        key[q] = k < cnt ? xu[XS * k] - u0 : 0;
+                        rank[q] = k < cnt ? atomicAdd(&s_ucnt[key[q]], 1) : 0;
+                    }
+                    __syncthreads();
+                    if (warp == 0) {   // exclusive scan of the counts; the counts join s_cu and are zeroed for the next tile
+                        const int per = (rows + 31) / 32, b0 = min(rows, lane * per), b1 = min(rows, b0 + per);
+                        int run = 0;
+                        for (int b = b0; b < b1; ++b) run += s_ucnt[b];
+                        int incl = run;
+#pragma unroll
+                        for (int off = 1; off < 32; off <<= 1) {
+                            const int y = __shfl_up_sync(0xffffffffu, incl, off);
+                            if (lane >= off) incl += y;
+                        }
+                        int start = incl - run;
+                        for (int b = b0; b < b1; ++b) {
+                            const int c = s_ucnt[b];
+                            s_uoff[b] = start;
+                            s_cu[b] += (unsigned)c;
+                            s_ucnt[b] = 0;
+                            start += c;
+                        }
+                        if (lane == 31) s_uoff[rows] = incl;
+                    }
+                    __syncthreads();
+#pragma unroll
+                    for (int q = 0; q < PT; ++q) {
+                        const int k = tid + q * kThreads;
+                        if (k < cnt) s_perm[s_uoff[key[q]] + rank[q]] = (uint16_t)k;
+                    }
+                    __syncthreads();
+                    span = (cnt + GROUPS - 1) / GROUPS;   // every group takes the same trip count (pair_loss shuffles)
+                    lo = min(cnt, group * span);
+                    hi = min(cnt, lo + span);
+                }
+            }
+            // UBK: add the run sum of local user urun to its accumulator row (every lane of the group, its own chunks)
+            auto flush = [&]() {
+                if (urun < 0) return;
+                float *d = s_gp + urun * RS;
+                const bool own = s_uoff[urun] >= lo && s_uoff[urun + 1] <= hi;
+#pragma unroll
+                for (int ch = 0; ch < NCH; ++ch) {
+                    const int cc = gl + ch * W;
+                    if (cc >= chunks) continue;
+                    float4 *d4 = reinterpret_cast<float4 *>(d + cc * VEC);
+                    if (own) {
+                        float4 x = *d4;
+                        x.x += ua[ch].v[0]; x.y += ua[ch].v[1]; x.z += ua[ch].v[2]; x.w += ua[ch].v[3];
+                        *d4 = x;
+                    } else {
+#pragma unroll
+                        for (int e = 0; e < VEC; ++e) atomicAdd(d + cc * VEC + e, ua[ch].v[e]);
+                    }
+                }
+            };
 
-            for (int tb = 0; tb < cnt; tb += GROUPS * UNR) {
+            for (int tb = 0; tb < (sorted ? span : cnt); tb += (sorted ? UNR : GROUPS * UNR)) {
                 Row<VEC, W, NCH> rp[UNR], rqi[UNR], rqj[UNR];
                 int iu[UNR], ii[UNR], ij[UNR];
                 RowOff ou[UNR], oi[UNR], oj[UNR];   // element offsets of the three rows (tables and accumulators alike)
@@ -550,6 +660,10 @@ __device__ __forceinline__ void bpr_steps_body(StepParams &p, XCH &xch)
                 for (int r = 0; r < UNR; ++r) {
                     int t = tb + r * GROUPS + group;
                     ok[r] = t < cnt;
+                    if (sorted) {
+                        ok[r] = lo + tb + r < hi;
+                        t = ok[r] ? s_perm[lo + tb + r] : 0;
+                    }
                     iu[r] = ok[r] ? xu[XS * t] : 0;
                     ii[r] = ok[r] ? xi[XS * t] : 0;
                     ij[r] = ok[r] ? xj[XS * t] : 0;
@@ -661,7 +775,7 @@ __device__ __forceinline__ void bpr_steps_body(StepParams &p, XCH &xch)
                 for (int r = 0; r < UNR; ++r) {
                     if (!ok[r]) continue;
                     const float c = cs[r];
-                    if (has_reg) {
+                    if (has_reg && !unorm) {   // unorm: the partition has summed the batch norms from the norm cache
                         float l1u = 0, l1i = 0, l1j = 0, s2u = 0, s2i = 0, s2j = 0;
                         Row<VEC, W, NCH> nu_ = rp[r], ni_ = rqi[r], nj_ = rqj[r];
                         if (!LEAN && p.Pn != nullptr) {   // regulariser on the ego rows (LightGCNRecommender.py:145-146,159)
@@ -678,11 +792,21 @@ __device__ __forceinline__ void bpr_steps_body(StepParams &p, XCH &xch)
                                 l1i += fabsf(b); s2i = fmaf(b, b, s2i);
                                 l1j += fabsf(d); s2j = fmaf(d, d, s2j);
                             }
-                        if (!unorm) { t_l1u += l1u; t_s2u += s2u; }   // unorm: the partition has summed the user norms
+                        t_l1u += l1u; t_s2u += s2u;
                         t_l1i += l1i; t_l1j += l1j;
                         t_s2i += s2i; t_s2j += s2j;
                     }
                     if (p.apply) {
+                        if constexpr (UBK && STAGED) {
+                            if (iu[r] - u0 != urun) {   // a new run: flush the last one
+                                flush();
+                                urun = iu[r] - u0;
+#pragma unroll
+                                for (int ch = 0; ch < NCH; ++ch)
+#pragma unroll
+                                    for (int e = 0; e < VEC; ++e) ua[ch].v[e] = 0.f;
+                            }
+                        }
 #pragma unroll
                         for (int ch = 0; ch < NCH; ++ch) {
                             int cc = gl + ch * W;
@@ -694,6 +818,10 @@ __device__ __forceinline__ void bpr_steps_body(StepParams &p, XCH &xch)
                                     gu.v[e] = c * (rqi[r].c[ch].v[e] - rqj[r].c[ch].v[e]);
                                     gi.v[e] = c * rp[r].c[ch].v[e];
                                     gj.v[e] = -gi.v[e];
+                                    if (UBK && unorm) {   // the item rows' regulariser, once per occurrence (no counters)
+                                        gi.v[e] += reg_term(rqi[r].c[ch].v[e], s_inv[1], p);
+                                        gj.v[e] += reg_term(rqj[r].c[ch].v[e], s_inv[2], p);
+                                    }
                                 } else {
                                     gu.v[e] = c * rqi[r].c[ch].v[e] + cn[r] * rqj[r].c[ch].v[e];
                                     gi.v[e] = c * rp[r].c[ch].v[e];
@@ -708,8 +836,11 @@ __device__ __forceinline__ void bpr_steps_body(StepParams &p, XCH &xch)
                                     if (!pw) det_red(p.ws.gQ64 + oj[r] + cc * VEC + e, gj.v[e]);
                                 }
                             } else {
-                                if constexpr (UBK) {
-                                    float *d = s_gp + (iu[r] - u0) * (F + 1) + cc * VEC;
+                                if constexpr (UBK && STAGED) {
+#pragma unroll
+                                    for (int e = 0; e < VEC; ++e) ua[ch].v[e] += gu.v[e];
+                                } else if constexpr (UBK) {
+                                    float *d = s_gp + (iu[r] - u0) * RS + cc * VEC;
 #pragma unroll
                                     for (int e = 0; e < VEC; ++e) atomicAdd(d + e, gu.v[e]);
                                 } else {
@@ -720,11 +851,17 @@ __device__ __forceinline__ void bpr_steps_body(StepParams &p, XCH &xch)
                             }
                         }
                         if (gl == 0) {
-                            if constexpr (UBK) atomicAdd(s_cu + (iu[r] - u0), 1u);
-                            else if (GEN && p.U == 0) red_add_u64(p.ws.cntI + iu[r], 1ull);
-                            else red_add_u32(p.ws.cntU + iu[r], 1u);
-                            red_add_u64(p.ws.cntI + ii[r], 1ull);
-                            if (!pw) red_add_u64(p.ws.cntI + ij[r], 1ull << 32);
+                            if constexpr (UBK) {
+                                if (!sorted) atomicAdd(s_cu + (iu[r] - u0), 1u);   // sorted: the tile's sort has counted it
+                            } else if (GEN && p.U == 0) {
+                                red_add_u64(p.ws.cntI + iu[r], 1ull);
+                            } else {
+                                red_add_u32(p.ws.cntU + iu[r], 1u);
+                            }
+                            if (!(UBK && ustage)) {   // ustage: the item sweep needs no counters
+                                red_add_u64(p.ws.cntI + ii[r], 1ull);
+                                if (!pw) red_add_u64(p.ws.cntI + ij[r], 1ull << 32);
+                            }
                             if (GEN && p.bias != nullptr) {   // d loss / d (u_bias, i_bias, bias_): no regulariser (:76-95)
                                 const float cboth = pw ? c : c + cn[r];
                                 asm volatile("red.relaxed.gpu.global.add.f32 [%0], %1;" ::"l"(p.ws.gB + iu[r]), "f"(cboth) : "memory");
@@ -737,6 +874,7 @@ __device__ __forceinline__ void bpr_steps_body(StepParams &p, XCH &xch)
                     }
                 }
             }
+            if constexpr (UBK && STAGED) flush();
             // per-thread fp32 partials cover <= tile/GROUPS triples: warp-reduce, widen to fp64 in smem
             {
                 float tv[8] = {t_loss, t_l1u, t_l1i, t_l1j, t_s2u, t_s2i, t_s2j, t_gb0};
@@ -763,12 +901,12 @@ __device__ __forceinline__ void bpr_steps_body(StepParams &p, XCH &xch)
                         const bool live = k < n && s_cu[r] != 0u;
                         float4 th = make_float4(0.f, 0.f, 0.f, 0.f);
                         if (live) {
-                            const float *a = s_pu + r * F + c * VEC, *g = s_gp + r * (F + 1) + c * VEC;
+                            const float *a = s_pu + r * F + c * VEC, *g = s_gp + r * F + c * VEC;
                             const float cnt = (float)s_cu[r];
-                            th.x = a[0] - p.lr * reg_grad(a[0], p.gscale * g[0], cnt, inv_u, 0.f, 0.f, p);
-                            th.y = a[1] - p.lr * reg_grad(a[1], p.gscale * g[1], cnt, inv_u, 0.f, 0.f, p);
-                            th.z = a[2] - p.lr * reg_grad(a[2], p.gscale * g[2], cnt, inv_u, 0.f, 0.f, p);
-                            th.w = a[3] - p.lr * reg_grad(a[3], p.gscale * g[3], cnt, inv_u, 0.f, 0.f, p);
+                            th.x = a[0] - p.lr * reg_grad(a[0], p.gscale * g[0], cnt, s_inv[0], 0.f, 0.f, p);
+                            th.y = a[1] - p.lr * reg_grad(a[1], p.gscale * g[1], cnt, s_inv[0], 0.f, 0.f, p);
+                            th.z = a[2] - p.lr * reg_grad(a[2], p.gscale * g[2], cnt, s_inv[0], 0.f, 0.f, p);
+                            th.w = a[3] - p.lr * reg_grad(a[3], p.gscale * g[3], cnt, s_inv[0], 0.f, 0.f, p);
                             __stcg(reinterpret_cast<float4 *>(p.P + (size_t)(u0 + r) * F + c * VEC), th);
                         }
                         if (unorm) {
@@ -783,7 +921,7 @@ __device__ __forceinline__ void bpr_steps_body(StepParams &p, XCH &xch)
                     for (int k = tid; k < rows * chunks; k += kThreads) {
                         const int r = k / chunks, c = k - r * chunks;
                         if (s_cu[r] == 0u) continue;
-                        const float *a = s_gp + r * (F + 1) + c * VEC;
+                        const float *a = s_gp + r * RS + c * VEC;
                         __stcg(reinterpret_cast<float4 *>(p.ws.gP + (size_t)(u0 + r) * F + c * VEC), make_float4(a[0], a[1], a[2], a[3]));
                     }
                     for (int k = tid; k < rows; k += kThreads)
@@ -878,10 +1016,29 @@ __device__ __forceinline__ void bpr_steps_body(StepParams &p, XCH &xch)
                     else
                         dense_sweep<VEC, W, NCH, DRB_OPT_RMSPROP, false, true>(p, nm, ac, gl, group, GROUPS, chunks);
                 }
+            } else if (UBK && ustage) {
+                // the user rows took their update when their bucket completed, and phase 1 has added the item regulariser to
+                // gQ: every item row takes theta -= lr gQ (a zero chunk does not move), one chunk per thread, and rewrites its
+                // norm cache entry (the W * NCH chunks of a row on consecutive lanes)
+                constexpr int CH = W * NCH;
+                const long long nt = (long long)p.I * CH;
+                for (long long k0 = (long long)blockIdx.x * kThreads; k0 < nt; k0 += (long long)gridDim.x * kThreads) {
+                    const long long k = k0 + tid;
+                    float4 th = make_float4(0.f, 0.f, 0.f, 0.f), g = th;
+                    float4 *tp = reinterpret_cast<float4 *>(p.Q) + k, *gp = reinterpret_cast<float4 *>(p.ws.gQ) + k;
+                    if (k < nt) { th = __ldcg(tp); g = __ldcg(gp); }
+                    if (g.x != 0.f || g.y != 0.f || g.z != 0.f || g.w != 0.f) {
+                        th.x = th.x - p.lr * g.x; th.y = th.y - p.lr * g.y; th.z = th.z - p.lr * g.z; th.w = th.w - p.lr * g.w;
+                        __stcg(tp, th);
+                        __stcg(gp, make_float4(0.f, 0.f, 0.f, 0.f));
+                    }
+                    if (unorm) {
+                        const float2 nrm = row_norms<CH>(th);
+                        if (k < nt && k % CH == 0) __stcg(p.ub_norm + p.U + k / CH, nrm);
+                    }
+                }
             } else if (dense || p.opt != DRB_OPT_SGD) {   // stateful optimisers always sweep (claim mode is SGD only)
-                if (ustage)                        // the user rows took their update when their bucket completed
-                    dense_sweep<VEC, W, NCH, DRB_OPT_SGD, false, false, UBK>(p, nm, ac, gl, group, GROUPS, chunks);
-                else if (p.opt == DRB_OPT_SGD)
+                if (p.opt == DRB_OPT_SGD)
                     dense_sweep<VEC, W, NCH, DRB_OPT_SGD, XCH::kActive>(p, nm, ac, gl, group, GROUPS, chunks);
                 else if (p.opt == DRB_OPT_ADAM)
                     dense_sweep<VEC, W, NCH, DRB_OPT_ADAM, XCH::kActive>(p, nm, ac, gl, group, GROUPS, chunks);
@@ -985,11 +1142,11 @@ __global__ void __launch_bounds__(kThreads, DRB_MINB) mf_bpr_steps_kernel(StepPa
     bpr_steps_body<VEC, W, NCH, GEN, NoExchange>(p, x);
 }
 
-template <int VEC, int W, int NCH, bool UBK = false>
+template <int VEC, int W, int NCH, bool UBK = false, bool STAGED = false>
 __global__ void __launch_bounds__(kThreads, DRB_MINB) mf_bpr_steps_lean_kernel(StepParams p)
 {
     NoExchange x;
-    bpr_steps_body<VEC, W, NCH, false, NoExchange, true, UBK>(p, x);
+    bpr_steps_body<VEC, W, NCH, false, NoExchange, true, UBK, STAGED>(p, x);
 }
 
 // the conditions under which the lean body computes what the general one does
