@@ -15,7 +15,7 @@ LIBDIR = os.path.join(HERE, "lib")
 SO = os.path.join(LIBDIR, "libdaisyrec_b200.so")
 HEADER = os.path.join(os.path.dirname(HERE), "include", "daisyrec_b200.h")
 SOURCES = ["capi.cu", "mf_bpr.cu", "sampler.cu", "rank.cu", "shard.cu", "lightgcn.cu", "neumf.cu", "comm.cu", "metrics.cu", "csr.cu", "randperm.cu", "p2p.cu", "ngcf.cu", "nfm.cu",
-           "skipgram.cu", "item2vec.cu", "ease.cu", "itemknn.cu", "slim.cu", "puresvd.cu", "vae.cu"]
+           "skipgram.cu", "item2vec.cu", "ease.cu", "itemknn.cu", "userknn.cu", "mostpop.cu", "slim.cu", "puresvd.cu", "vae.cu"]
 ARCH = ["-gencode", "arch=compute_90a,code=sm_90a"]
 FLAGS = ["-O3", "-std=c++17", "-lineinfo", "-Xcompiler", "-fPIC", "--threads", "4"]
 

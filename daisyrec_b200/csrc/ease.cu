@@ -17,6 +17,10 @@
 //                     No floating-point atomics: each tile belongs to one CTA per chunk and chunks run in order, so G is
 //                     bitwise reproducible.  The exact path gives the exact Gram; it equals the reference's fp64 matrix
 //                     bit for bit while max_i sum_u (x_ui 2^s)^2 < 2^24, where scipy's fp32 sums are exact as well.
+//   drb_gram_image / drb_gram_panel   the same Gram by row panels, for UserKNN's [U, U] matrix that is never held whole:
+//                     one dense image of the CSR's columns over all of K (s8 or fp64 as above), then G[p0 .. p0 + rows, :]
+//                     on a rectangular tile grid that runs the triangle grid's tile body.  Each entry is one CTA's full-K
+//                     sum, so a panel's rows do not depend on the panel size.
 //   drb_ease_inverse  P = G^-1 in place by the blocked sweep operator (symmetric block Gauss-Jordan, no pivoting: G is
 //                     positive definite for reg > 0).  Per pivot block k of kNb columns:
 //                       D = G_kk^-1 in one CTA (scalar sweep in shared memory; a pivot <= 0 raises a sticky flag),
@@ -195,18 +199,18 @@ __device__ __forceinline__ void imma_m16n8k32(int (&d)[4], const int (&a)[4], co
                  : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "r"(b[0]), "r"(b[1]));
 }
 
-// G[tile bi, tile bj] += unit * (image rows of bi) . (image rows of bj)^T over the chunk's K columns; s8 x s8 -> s32.
-// 8 warps as 2 x 4, each 64 x 32 of the 128 x 128 tile: 4 x 4 fragments of m16n8k32.
-__global__ void __launch_bounds__(256) ease_gram_s8_kernel(const int8_t *__restrict__ img, long long ld, int K, double *__restrict__ G,
-                                                           int n, double unit)
+// Gt[r][c] += unit * (128 image rows at Ag) . (128 image rows at Bg)^T over K columns, for r < nr, c < nc (Gt: the tile's
+// origin in a row-major fp64 matrix of leading dimension ldg); s8 x s8 -> s32.  8 warps as 2 x 4, each 64 x 32 of the 128 x 128
+// tile: 4 x 4 fragments of m16n8k32.  One 256-thread CTA; the triangle grid below (kAdd: chunks accumulate) and the panel grid
+// (a single full-K pass that stores, so the panel needs no zeroing) share it.
+template <bool kAdd>
+__device__ __forceinline__ void gram_s8_tile(const int8_t *__restrict__ Ag, const int8_t *__restrict__ Bg, long long ld, int K,
+                                             double *__restrict__ Gt, long long ldg, int nr, int nc, double unit)
 {
     __shared__ __align__(16) int8_t As[kS8Tile][kS8K + 16];   // 80-byte rows: a fragment's 8 rows hit distinct banks
     __shared__ __align__(16) int8_t Bs[kS8Tile][kS8K + 16];
-    int bi, bj;
-    tri_pair(blockIdx.x, bi, bj);
     const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31, g = lane >> 2, t = lane & 3;
     const int wm = (warp >> 2) * 64, wn = (warp & 3) * 32;
-    const int8_t *Ag = img + (long long)bi * kS8Tile * ld, *Bg = img + (long long)bj * kS8Tile * ld;
     int acc[4][4][4];
 #pragma unroll
     for (int mi = 0; mi < 4; ++mi)
@@ -252,30 +256,71 @@ __global__ void __launch_bounds__(256) ease_gram_s8_kernel(const int8_t *__restr
         for (int ni = 0; ni < 4; ++ni)
 #pragma unroll
             for (int e = 0; e < 4; ++e) {
-                const int r = bi * kS8Tile + wm + mi * 16 + g + (e >> 1) * 8;
-                const int c = bj * kS8Tile + wn + ni * 8 + t * 2 + (e & 1);
-                if (r < n && c < n && acc[mi][ni][e] != 0) G[(long long)r * n + c] += (double)acc[mi][ni][e] * unit;
+                const int r = wm + mi * 16 + g + (e >> 1) * 8;
+                const int c = wn + ni * 8 + t * 2 + (e & 1);
+                if (r >= nr || c >= nc) continue;
+                if (!kAdd) Gt[(long long)r * ldg + c] = (double)acc[mi][ni][e] * unit;
+                else if (acc[mi][ni][e] != 0) Gt[(long long)r * ldg + c] += (double)acc[mi][ni][e] * unit;
             }
 }
 
-// general path: G[tile bi, tile bj] += (fp64 image rows of bi) . (rows of bj)^T on DMMA
-__global__ void __launch_bounds__(256) ease_gram_f64_kernel(const double *__restrict__ img, long long ld, int K, double *__restrict__ G,
-                                                            int n)
+// G[tile bi, tile bj] += unit * (image rows of bi) . (image rows of bj)^T over the chunk's K columns (lower triangle, bi >= bj)
+__global__ void __launch_bounds__(256) ease_gram_s8_kernel(const int8_t *__restrict__ img, long long ld, int K, double *__restrict__ G,
+                                                           int n, double unit)
 {
-    __shared__ DmmaSmem sm;
     int bi, bj;
     tri_pair(blockIdx.x, bi, bj);
+    gram_s8_tile<true>(img + (long long)bi * kS8Tile * ld, img + (long long)bj * kS8Tile * ld, ld, K,
+                 G + (long long)bi * kS8Tile * n + (long long)bj * kS8Tile, n, n - bi * kS8Tile, n - bj * kS8Tile, unit);
+}
+
+// general path: Gt[r][c] += (64 fp64 image rows at Ag) . (64 rows at Bg)^T on DMMA for r < nr, c < nc (as gram_s8_tile;
+// = when !kAdd)
+template <bool kAdd>
+__device__ __forceinline__ void gram_f64_tile(const double *__restrict__ Ag, const double *__restrict__ Bg, long long ld, int K,
+                                              double *__restrict__ Gt, long long ldg, int nr, int nc)
+{
+    __shared__ DmmaSmem sm;
     double acc[4][2][2] = {};
-    dmma_nt_64(img + (long long)bi * kDmmaTile * ld, ld, img + (long long)bj * kDmmaTile * ld, ld, K, acc, sm);
+    dmma_nt_64(Ag, ld, Bg, ld, K, acc, sm);
 #pragma unroll
     for (int mi = 0; mi < 4; ++mi)
 #pragma unroll
         for (int ni = 0; ni < 2; ++ni)
 #pragma unroll
             for (int e = 0; e < 2; ++e) {
-                const int r = bi * kDmmaTile + dmma_row(mi), c = bj * kDmmaTile + dmma_col(ni, e);
-                if (r < n && c < n) G[(long long)r * n + c] += acc[mi][ni][e];
+                const int r = dmma_row(mi), c = dmma_col(ni, e);
+                if (r < nr && c < nc) {
+                    if (kAdd) Gt[(long long)r * ldg + c] += acc[mi][ni][e];
+                    else Gt[(long long)r * ldg + c] = acc[mi][ni][e];
+                }
             }
+}
+
+// G[tile bi, tile bj] += (fp64 image rows of bi) . (rows of bj)^T (lower triangle)
+__global__ void __launch_bounds__(256) ease_gram_f64_kernel(const double *__restrict__ img, long long ld, int K, double *__restrict__ G,
+                                                            int n)
+{
+    int bi, bj;
+    tri_pair(blockIdx.x, bi, bj);
+    gram_f64_tile<true>(img + (long long)bi * kDmmaTile * ld, img + (long long)bj * kDmmaTile * ld, ld, K,
+                  G + (long long)bi * kDmmaTile * n + (long long)bj * kDmmaTile, n, n - bi * kDmmaTile, n - bj * kDmmaTile);
+}
+
+// rectangular grid (column tiles, row tiles): G[r][c] = image row (p0 + r) . image row c for r < rows, c < n (G: ldg = n)
+__global__ void __launch_bounds__(256) gram_panel_s8_kernel(const int8_t *__restrict__ img, long long ld, int K, int p0, int rows,
+                                                            int n, double *__restrict__ G, double unit)
+{
+    const int r0 = blockIdx.y * kS8Tile, c0 = blockIdx.x * kS8Tile;
+    gram_s8_tile<false>(img + (long long)(p0 + r0) * ld, img + (long long)c0 * ld, ld, K, G + (long long)r0 * n + c0, n, rows - r0, n - c0,
+                 unit);
+}
+
+__global__ void __launch_bounds__(256) gram_panel_f64_kernel(const double *__restrict__ img, long long ld, int K, int p0, int rows,
+                                                             int n, double *__restrict__ G)
+{
+    const int r0 = blockIdx.y * kDmmaTile, c0 = blockIdx.x * kDmmaTile;
+    gram_f64_tile<false>(img + (long long)(p0 + r0) * ld, img + (long long)c0 * ld, ld, K, G + (long long)r0 * n + c0, n, rows - r0, n - c0);
 }
 
 // upper triangle := lower triangle; diagonal += reg (fp64, rounded once as scipy's G + reg * identity)
@@ -580,6 +625,57 @@ extern "C" int drb_ease_gram(const int64_t *d_row_ptr, const int32_t *d_col, con
         DRB_CUDA(cudaGetLastError());
     }
     ease_mirror_kernel<<<grid_for((long long)n * n, 256), 256, 0, st>>>(d_G, n, reg);
+    DRB_CUDA(cudaGetLastError());
+    return DRB_OK;
+}
+
+// the whole-K image of drb_gram_image: rows = the CSR's columns padded to the s8 tile, ld = its rows padded to the K step
+static void panel_geom(int K, int n, long long &rows, long long &ld)
+{
+    rows = round_up(n, kS8Tile);
+    ld = round_up(K, kS8K);
+}
+
+extern "C" size_t drb_gram_image_bytes(int32_t k_rows, int32_t n, int32_t scale)
+{
+    if (k_rows <= 0 || n <= 0) return 0;
+    long long rows, ld;
+    panel_geom(k_rows, n, rows, ld);
+    return (size_t)(rows * ld * (scale >= 0 ? 1 : 8));
+}
+
+extern "C" int drb_gram_image(const int64_t *d_row_ptr, const int32_t *d_col, const float *d_val, int32_t k_rows, int32_t n,
+                              int32_t scale, void *d_img, void *stream)
+{
+    DRB_REQUIRE(d_row_ptr && d_img && k_rows > 0 && n > 0 && scale <= 7, "gram_image: bad arguments");
+    cudaStream_t st = (cudaStream_t)stream;
+    long long rows, ld;
+    panel_geom(k_rows, n, rows, ld);
+    DRB_CUDA(cudaMemsetAsync(d_img, 0, drb_gram_image_bytes(k_rows, n, scale), st));
+    const int grid = grid_for((long long)k_rows * 32, 256);
+    if (scale >= 0)
+        ease_image_kernel<int8_t><<<grid, 256, 0, st>>>(d_row_ptr, d_col, d_val, 0, k_rows, ld, (float)(1 << scale), (int8_t *)d_img);
+    else
+        ease_image_kernel<double><<<grid, 256, 0, st>>>(d_row_ptr, d_col, d_val, 0, k_rows, ld, 1.f, (double *)d_img);
+    DRB_CUDA(cudaGetLastError());
+    return DRB_OK;
+}
+
+extern "C" int drb_gram_panel(const void *d_img, int32_t k_rows, int32_t n, int32_t scale, int32_t p0, int32_t rows, double *d_G,
+                              void *stream)
+{
+    DRB_REQUIRE(d_img && d_G && k_rows > 0 && n > 0 && scale <= 7 && p0 >= 0 && p0 % kS8Tile == 0 && rows > 0 && p0 + rows <= n,
+                "gram_panel: bad arguments (p0 a multiple of %d, p0 + rows <= n)", kS8Tile);
+    cudaStream_t st = (cudaStream_t)stream;
+    long long prow, ld;
+    panel_geom(k_rows, n, prow, ld);
+    const int T = scale >= 0 ? kS8Tile : kDmmaTile;
+    const dim3 grid((unsigned)((n + T - 1) / T), (unsigned)((rows + T - 1) / T));
+    DRB_REQUIRE(grid.y <= 65535, "gram_panel: %d rows exceed the tile grid", rows);
+    if (scale >= 0)
+        gram_panel_s8_kernel<<<grid, 256, 0, st>>>((const int8_t *)d_img, ld, (int)ld, p0, rows, n, d_G, ldexp(1.0, -2 * scale));
+    else
+        gram_panel_f64_kernel<<<grid, 256, 0, st>>>((const double *)d_img, ld, (int)ld, p0, rows, n, d_G);
     DRB_CUDA(cudaGetLastError());
     return DRB_OK;
 }

@@ -9,7 +9,8 @@
 //                           pearson; every stored value 1: jaccard / tanimoto / dice / tversky) and ss_i, the fp32 sum of
 //                           x'^2 over item i's stored entries (its square root for the cosine family).  Every sum runs in
 //                           fp32 over ascending users / items, the order scipy's products add in.
-//   drb_itemknn_neighbours  one CTA per column j reads row j of G (G is symmetric) and keeps the min(maxk, I) largest weights
+//   drb_itemknn_neighbours  one CTA per column j reads row j of G (G is symmetric; drb_knn_neighbours_panel takes the rows
+//                           j0 .. j0 + rows of G as a panel, which is how UserKNN's [U, U] Gram is consumed) and keeps the min(maxk, I) largest weights
 //                           by (weight descending, item id ascending), drops exact zeros and stores the rest by ascending
 //                           item id.  Each weight is a few correctly rounded fp32 operations written with the _rn
 //                           intrinsics, evaluated left to right as numpy does, so nothing is contracted into an FMA.  The
@@ -145,16 +146,18 @@ __device__ __forceinline__ int block_flag_rank(bool flag, int *s_warp, int &tota
     return before + __popc(bal & ((1u << lane) - 1u));
 }
 
-__global__ void __launch_bounds__(kSelThreads) knn_select_kernel(const double *__restrict__ G, int n, const float *__restrict__ ss,
-                                                                 const KnnSim p, int keep, int maxk, int32_t *__restrict__ nbr_idx,
-                                                                 float *__restrict__ nbr_val, int32_t *__restrict__ nbr_cnt)
+// one CTA per row of a panel of G: row r holds column j = j0 + r (G is symmetric), ld entries apart
+__global__ void __launch_bounds__(kSelThreads) knn_select_kernel(const double *__restrict__ G, long long ld, int j0, int n,
+                                                                 const float *__restrict__ ss, const KnnSim p, int keep, int maxk,
+                                                                 int32_t *__restrict__ nbr_idx, float *__restrict__ nbr_val,
+                                                                 int32_t *__restrict__ nbr_cnt)
 {
     __shared__ unsigned hist[kSelBins];
     __shared__ int s_warp[kSelThreads / 32];
     __shared__ unsigned s_prefix;
     __shared__ int s_need;
-    const int j = blockIdx.x, tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
-    const double *row = G + (long long)j * n;
+    const int j = j0 + blockIdx.x, tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+    const double *row = G + (long long)blockIdx.x * ld;
     const float ssj = ss[j];
 
     // radix select: after the three passes `prefix` is the key of the keep-th largest weight and `need` how many weights
@@ -290,18 +293,26 @@ extern "C" int drb_itemknn_transform(const int64_t *d_row_ptr, const float *d_va
     return DRB_OK;
 }
 
+extern "C" int drb_knn_neighbours_panel(const double *d_G, int32_t n, int32_t j0, int32_t rows, const float *d_ss, int32_t family,
+                                        int32_t normalize, float shrink, int32_t maxk, int32_t *d_nbr_idx, float *d_nbr_val,
+                                        int32_t *d_nbr_cnt, void *stream)
+{
+    DRB_REQUIRE(d_G && d_ss && d_nbr_idx && d_nbr_val && d_nbr_cnt && n > 0 && j0 >= 0 && rows >= 0 && j0 + rows <= n &&
+                    family >= kKnnCosine && family <= kKnnTversky && maxk >= 1 && maxk <= 1024,
+                "itemknn_neighbours: bad arguments (maxk in [1, 1024])");
+    if (rows == 0) return DRB_OK;
+    const KnnSim p = {family, family == kKnnCosine ? normalize : 0, shrink};
+    knn_select_kernel<<<rows, kSelThreads, 0, (cudaStream_t)stream>>>(d_G, n, j0, n, d_ss, p, maxk < n ? maxk : n, maxk, d_nbr_idx,
+                                                                      d_nbr_val, d_nbr_cnt);
+    DRB_CUDA(cudaGetLastError());
+    return DRB_OK;
+}
+
 extern "C" int drb_itemknn_neighbours(const double *d_G, int32_t n, const float *d_ss, int32_t family, int32_t normalize,
                                       float shrink, int32_t maxk, int32_t *d_nbr_idx, float *d_nbr_val, int32_t *d_nbr_cnt,
                                       void *stream)
 {
-    DRB_REQUIRE(d_G && d_ss && d_nbr_idx && d_nbr_val && d_nbr_cnt && n > 0 && family >= kKnnCosine && family <= kKnnTversky &&
-                    maxk >= 1 && maxk <= 1024,
-                "itemknn_neighbours: bad arguments (maxk in [1, 1024])");
-    const KnnSim p = {family, family == kKnnCosine ? normalize : 0, shrink};
-    knn_select_kernel<<<n, kSelThreads, 0, (cudaStream_t)stream>>>(d_G, n, d_ss, p, maxk < n ? maxk : n, maxk, d_nbr_idx, d_nbr_val,
-                                                                   d_nbr_cnt);
-    DRB_CUDA(cudaGetLastError());
-    return DRB_OK;
+    return drb_knn_neighbours_panel(d_G, n, 0, n, d_ss, family, normalize, shrink, maxk, d_nbr_idx, d_nbr_val, d_nbr_cnt, stream);
 }
 
 extern "C" int drb_itemknn_scores(const int64_t *d_row_ptr, const int32_t *d_col, const float *d_val, const int32_t *d_nbr_idx,

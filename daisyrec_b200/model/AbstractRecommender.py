@@ -243,24 +243,32 @@ class DeviceRecommender(AbstractRecommender):
 
 
 class NeighbourScorer(DeviceRecommender):
-    """The item-item models whose prediction is X W with W kept as at most ``maxk`` neighbours per item (ops.KnnNeighbours):
-    ItemKNNCF and SLiM.  Subclasses set ``self._X`` (ops.EaseX), ``self._W`` and ``self._w_host = None`` in ``fit``.  Entries of
+    """The neighbourhood models whose prediction is a product with W kept as at most ``maxk`` neighbours per column
+    (ops.KnnNeighbours): ItemKNNCF and SLiM (X W), and UserKNNCF (W X, through ``_scoring``).  Subclasses set ``self._X`` (ops.EaseX), ``self._W`` and ``self._w_host = None`` in ``fit``.  Entries of
     X W are summed on demand in fp64 over ascending neighbour ids, the order scipy's product adds in; the product itself is not
     materialised."""
 
-    def _neighbour_csc(self):
-        """W as scipy csc_matrix float32 [I, I], column c holding the neighbours of item c (None before fit)."""
+    def _neighbour_csc(self, n=None):
+        """W as scipy csc_matrix float32 [n, n] (n: item_num unless given), column c holding the neighbours of c (None before
+        fit)."""
         if self._W is None:
             return None
         import scipy.sparse as sp
+        n = self.item_num if n is None else n
         cnt = self._W.cnt.cpu().numpy().astype(np.int64)
         keep = np.arange(self._W.maxk)[None, :] < cnt[:, None]
         return sp.csc_matrix((self._W.val.cpu().numpy()[keep], self._W.idx.cpu().numpy()[keep],
-                              np.concatenate([[0], np.cumsum(cnt)])), shape=(self.item_num, self.item_num))
+                              np.concatenate([[0], np.cumsum(cnt)])), shape=(n, n))
+
+    def _scoring(self):
+        """(the neighbour structure, rank op, full_rank op, predict op) the scoring methods call: W's forward lists with the
+        ItemKNN scoring kernels; UserKNNCF, whose product sums over reverse neighbours, supplies its own."""
+        return self._W, ops.itemknn_rank, ops.itemknn_full_rank, ops.itemknn_predict
 
     def _predict_score(self, u, i):
         us, its = self._ids((u,), (i,))
-        return np.float64(ops.itemknn_predict(self._X, self._W, us, its).item())
+        nb, _, _, predict = self._scoring()
+        return np.float64(predict(self._X, nb, us, its).item())
 
     def rank(self, test_loader):
         """-> int64 ndarray [n_test_users, topk] of candidate ids by (X W)[u, c], ties by candidate position; None for an empty
@@ -270,13 +278,14 @@ class NeighbourScorer(DeviceRecommender):
             return None
         users, cands, k = ins
         self._ids(())
-        return ops.itemknn_rank(self._X, self._W, torch.from_numpy(users).to(self.device),
-                                torch.from_numpy(cands).to(self.device), k).cpu().numpy()
+        nb, rank, _, _ = self._scoring()
+        return rank(self._X, nb, torch.from_numpy(users).to(self.device), torch.from_numpy(cands).to(self.device), k).cpu().numpy()
 
     def full_rank(self, u):
         """-> int64 ndarray [topk] of the top items of user u; no masking of train items."""
         users = self._ids((u,))[0]
-        return ops.itemknn_full_rank(self._X, self._W, users, min(self.topk, self.item_num))[0].cpu().numpy()
+        nb, _, full_rank, _ = self._scoring()
+        return full_rank(self._X, nb, users, min(self.topk, self.item_num))[0].cpu().numpy()
 
     def _ids(self, users, items=None):
         if self._W is None:

@@ -6,7 +6,8 @@ from .NGCFRecommender import NGCF  # noqa: F401
 from .NFMRecommender import NFM  # noqa: F401
 from .Item2VecRecommender import Item2Vec  # noqa: F401
 from .EASERecommender import EASE  # noqa: F401
-from .KNNCFRecommender import ItemKNNCF  # noqa: F401
+from .KNNCFRecommender import ItemKNNCF, UserKNNCF  # noqa: F401
+from .PopRecommender import MostPop  # noqa: F401
 from .SLiMRecommender import SLiM  # noqa: F401
 from .PureSVDRecommender import PureSVD  # noqa: F401
 from .VAECFRecommender import VAECF  # noqa: F401

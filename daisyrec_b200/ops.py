@@ -958,6 +958,170 @@ def itemknn_predict(X, W, users, items):
     return itemknn_scores(X, W, users, items.reshape(-1, 1)).reshape(-1)
 
 
+# ------------------------------------------------------------------ UserKNN
+USERKNN_PANEL_BYTES = 1 << 32          # the largest Gram panel userknn_neighbours allocates (fp64 [rows, U])
+
+
+def userknn_transform(X, d_u, d_i, similarity):
+    """The similarity's view of X^T [I, U], whose columns are users (KNNCFRecommender.py:491-497) -> (EaseX of X^T with the
+    transformed values (rows = items, user_num = I, item_num = U) and its own exact-Gram scale, ss float32 [U]).  adjusted
+    removes each item's mean, pearson each user's.  X^T is drb_csr_build of the train COO (d_u, d_i int32) with X's values."""
+    transform, _, root = KNN_SIMILARITY[similarity]
+    U, I, dev, nnz = X.user_num, X.item_num, X.val.device, X.col.numel()
+    t_ptr, t_col = csr_build(d_i, d_u, I, U)
+    assert t_col.numel() == nnz
+    t_val = torch.empty(max(nnz, 1), dtype=torch.float32, device=dev)
+    order = torch.empty(max(nnz, 1), dtype=torch.int32, device=dev)
+    L.check(L.lib().drb_userknn_transpose(_ptr(X.row_ptr), _ptr(X.col), _ptr(X.val), U, _ptr(t_ptr), _ptr(t_col), _ptr(t_val),
+                                          _ptr(order), _stream()))
+    val = torch.empty(max(nnz, 1), dtype=torch.float32, device=dev)
+    ss = torch.empty(U, dtype=torch.float32, device=dev)
+    L.check(L.lib().drb_itemknn_transform(_ptr(t_ptr), _ptr(t_val), I, U, _ptr(X.row_ptr), _ptr(order), transform, root, _ptr(val),
+                                          _ptr(ss), _stream()))
+    del t_val, order
+    ws = torch.empty(L.lib().drb_ease_csr_workspace_bytes(U, 0), dtype=torch.uint8, device=dev)
+    scale = C.c_int32(0)
+    L.check(L.lib().drb_ease_scale(_ptr(t_ptr), _ptr(t_col), _ptr(val), I, U, _ptr(ws), C.byref(scale), _stream()))
+    return EaseX(t_ptr, t_col.contiguous(), val[:nnz], int(scale.value), I, U), ss
+
+
+def gram_image(Xt):
+    """Dense image of Xt's columns over all of its rows (s8 x 2^scale when Xt.scale >= 0, else fp64) -> uint8 buffer."""
+    img = torch.empty(L.lib().drb_gram_image_bytes(Xt.user_num, Xt.item_num, Xt.scale), dtype=torch.uint8, device=Xt.val.device)
+    L.check(L.lib().drb_gram_image(_ptr(Xt.row_ptr), _ptr(Xt.col), _ptr(Xt.val), Xt.user_num, Xt.item_num, Xt.scale, _ptr(img),
+                                   _stream()))
+    return img
+
+
+def gram_panel(img, Xt, p0, rows, out=None):
+    """Rows p0 .. p0 + rows - 1 of Xt^T Xt, fp64 [rows, n] (p0 a multiple of 128), from gram_image(Xt)."""
+    n = Xt.item_num
+    G = torch.empty((rows, n), dtype=torch.float64, device=img.device) if out is None else out[:rows * n].view(rows, n)
+    L.check(L.lib().drb_gram_panel(_ptr(img), Xt.user_num, n, Xt.scale, p0, rows, _ptr(G), _stream()))
+    return G
+
+
+def userknn_panel_rows(user_num, free_bytes):
+    """Users per Gram panel: a multiple of 128, at most USERKNN_PANEL_BYTES and ``free_bytes`` of fp64 rows (0: none fits)."""
+    cap = min(free_bytes, USERKNN_PANEL_BYTES) // (8 * user_num) // 128 * 128
+    return int(min(cap, (user_num + 127) // 128 * 128))
+
+
+def userknn_neighbours(Xt, ss, similarity, normalize, shrink, maxk, panel):
+    """compute_similarity's column loop on X^T: per user column j the min(maxk, U) largest weights by (weight descending, id
+    ascending), exact zeros dropped -> KnnNeighbours [U, maxk].  The [U, U] Gram is formed ``panel`` rows at a time (a
+    multiple of 128) and each panel's rows are selected before the next is formed."""
+    n = Xt.item_num
+    if panel <= 0 or panel % 128:
+        raise ValueError(f'userknn_neighbours: panel must be a positive multiple of 128, got {panel}')
+    dev = Xt.val.device
+    idx = torch.empty((n, maxk), dtype=torch.int32, device=dev)
+    val = torch.empty((n, maxk), dtype=torch.float32, device=dev)
+    cnt = torch.empty(n, dtype=torch.int32, device=dev)
+    img = gram_image(Xt)
+    rows = min(panel, n)
+    buf = torch.empty(rows * n, dtype=torch.float64, device=dev)
+    family = KNN_SIMILARITY[similarity][1]
+    for p0 in range(0, n, panel):
+        r = min(panel, n - p0)
+        G = gram_panel(img, Xt, p0, r, buf)
+        L.check(L.lib().drb_knn_neighbours_panel(_ptr(G), n, p0, r, _ptr(ss), family, int(bool(normalize)), float(np.float32(shrink)),
+                                                 maxk, _ptr(idx), _ptr(val), _ptr(cnt), _stream()))
+    return KnnNeighbours(idx, val, cnt)
+
+
+class KnnReverse:
+    """R(u) = {v : u in N(v)} as a CSR over u: r_ptr int64 [U+1], r_col int32 (ascending v), r_val float32 = W[u, v]."""
+
+    def __init__(self, r_ptr, r_col, r_val):
+        self.r_ptr, self.r_col, self.r_val = r_ptr, r_col, r_val
+
+
+def userknn_reverse(W):
+    """Forward lists (KnnNeighbours, column v = N(v)) -> KnnReverse."""
+    n, maxk = W.idx.shape
+    dev = W.idx.device
+    pu = torch.empty(n * maxk, dtype=torch.int32, device=dev)
+    pv = torch.empty(n * maxk, dtype=torch.int32, device=dev)
+    L.check(L.lib().drb_userknn_pairs(_ptr(W.idx), _ptr(W.cnt), n, maxk, _ptr(pu), _ptr(pv), _stream()))
+    r_ptr, r_col = csr_build(pu, pv, n + 1, n)
+    del pu, pv
+    r_ptr = r_ptr[:n + 1].contiguous()
+    nnz = int(r_ptr[n].item())
+    r_col = r_col[:nnz].contiguous()
+    r_val = torch.empty(max(nnz, 1), dtype=torch.float32, device=dev)
+    L.check(L.lib().drb_userknn_place(_ptr(W.idx), _ptr(W.val), _ptr(W.cnt), n, maxk, _ptr(r_ptr), _ptr(r_col), _ptr(r_val),
+                                      _stream()))
+    return KnnReverse(r_ptr, r_col, r_val[:nnz])
+
+
+def userknn_scores(X, R, users, cands=None):
+    """pred_mat[u, c] = sum_{v in R(u)} W[u, v] x_vc in fp64 over ascending v -> [n, C] for ``cands`` int64 [n, C], or [n, I]
+    over every item."""
+    _dev(users, torch.int64, "users")
+    n = users.numel()
+    if cands is None:
+        sc = torch.empty((n, X.item_num), dtype=torch.float64, device=users.device)
+        L.check(L.lib().drb_userknn_full_scores(_ptr(X.row_ptr), _ptr(X.col), _ptr(X.val), _ptr(R.r_ptr), _ptr(R.r_col), _ptr(R.r_val),
+                                                X.item_num, _ptr(users), n, _ptr(sc), _stream()))
+        return sc
+    _dev(cands, torch.int64, "cands")
+    sc = torch.empty((n, cands.shape[1]), dtype=torch.float64, device=users.device)
+    L.check(L.lib().drb_userknn_scores(_ptr(X.row_ptr), _ptr(X.col), _ptr(X.val), _ptr(R.r_ptr), _ptr(R.r_col), _ptr(R.r_val),
+                                       _ptr(users), n, _ptr(cands), cands.shape[1], _ptr(sc), _stream()))
+    return sc
+
+
+def userknn_rank(X, R, users, cands, topk, scores=False):
+    """-> int64 [n, topk] candidate ids by (score descending, candidate position ascending) (and the scores when asked)."""
+    sc = userknn_scores(X, R, users, cands)
+    out = _itemknn_topk(sc, cands, topk)
+    return (out, sc) if scores else out
+
+
+def userknn_full_rank(X, R, users, topk, scores=False):
+    """-> int64 [n, topk] item ids by (score descending, id ascending) over every item (and the scores when asked)."""
+    sc = userknn_scores(X, R, users)
+    out = _itemknn_topk(sc, None, topk)
+    return (out, sc) if scores else out
+
+
+def userknn_predict(X, R, users, items):
+    """-> fp64 [n]: pred_mat[u, i] per (u, i) pair."""
+    _dev(items, torch.int64, "items")
+    return userknn_scores(X, R, users, items.reshape(-1, 1).contiguous()).reshape(-1)
+
+
+# ------------------------------------------------------------------ MostPop
+def mostpop_fit(d_ids, item_num):
+    """value_counts of the item ids (int64, every row) -> (cnt fp64 [I], score fp64 [I] = cnt / (1 + cnt)).  IndexError when
+    an id is outside [0, item_num)."""
+    _dev(d_ids, torch.int64, "ids")
+    dev = d_ids.device
+    ws = torch.empty(L.lib().drb_mostpop_workspace_bytes(item_num), dtype=torch.uint8, device=dev)
+    cnt = torch.empty(item_num, dtype=torch.float64, device=dev)
+    score = torch.empty(item_num, dtype=torch.float64, device=dev)
+    bad = C.c_int64(0)
+    L.check(L.lib().drb_mostpop_fit(_ptr(d_ids), d_ids.numel(), item_num, _ptr(ws), _ptr(cnt), _ptr(score), C.byref(bad), _stream()))
+    if bad.value:
+        raise IndexError(f'index out of range: {bad.value} item id(s) outside [0, {item_num})')
+    return cnt, score
+
+
+def mostpop_rank(score, cands, topk):
+    """-> int64 [n, topk] candidate ids by (score descending, candidate position ascending)."""
+    _dev(score, torch.float64, "score"); _dev(cands, torch.int64, "cands")
+    sc = torch.empty(cands.shape, dtype=torch.float64, device=cands.device)
+    L.check(L.lib().drb_mostpop_gather(_ptr(score), _ptr(cands), cands.numel(), _ptr(sc), _stream()))
+    return _itemknn_topk(sc, cands, topk)
+
+
+def mostpop_order(score, topk):
+    """-> int64 [topk] item ids by (score descending, id ascending)."""
+    _dev(score, torch.float64, "score")
+    return _itemknn_topk(score.view(1, -1), None, topk)[0]
+
+
 # ------------------------------------------------------------------ SLiM
 class SlimPanel:
     """drb_slim_solve's result for targets begin .. begin + count - 1 (row r = item begin + r): the live coordinates lidx int32

@@ -563,6 +563,59 @@ int drb_itemknn_scores(const int64_t *d_row_ptr, const int32_t *d_col, const flo
 int drb_itemknn_topk(const double *d_scores, int64_t n_rows, int32_t cand_num, const int64_t *d_cands, int32_t topk,
                      int64_t *d_out, void *stream);
 
+/* ---- UserKNN: daisy/model/KNNCFRecommender.py (UserKNNCF, :459-536), csrc/userknn.cu + the panel entry points of ease.cu /
+ * itemknn.cu.  The similarity is ItemKNN's on X^T [I, U], so W is [U, U] (column j: the neighbours of user j) and
+ * pred_mat = W X (:510), a sum over each user's reverse neighbours.
+ * drb_gram_image          the dense image of a CSR with k_rows rows and n columns, over all of K: image row c = column c of the
+ *                         CSR (x 2^scale as s8 when scale >= 0, else fp64), rows padded to 128, K to 64.  d_img:
+ *                         drb_gram_image_bytes(k_rows, n, scale) bytes.  (Given X^T, the rows are users and K is the items.)
+ * drb_gram_panel          d_G fp64 [rows, n] = image rows p0 .. p0 + rows - 1 times the image's transpose: the Gram rows of
+ *                         drb_ease_gram (exact on the s8 path; fp64 DMMA otherwise), with p0 a multiple of 128.  Every entry
+ *                         is one full-K sum, so it does not depend on p0 or rows.
+ * drb_knn_neighbours_panel  drb_itemknn_neighbours for the columns j0 .. j0 + rows - 1 of an [n, n] Gram matrix of which d_G
+ *                         holds those rows ([rows, n], row r = column j0 + r); writes rows j0 .. of the neighbour arrays.
+ * drb_userknn_transpose   for each slot k of X (CSR, user_num rows) of item i and user u: pos = the slot of u in row i of X^T
+ *                         (d_t_ptr / d_t_col: drb_csr_build of the (item, user) pairs), d_t_val[pos] = d_val[k],
+ *                         d_order[k] = pos.  X's row pointer and d_order group X^T's slots by user, items ascending.
+ * drb_userknn_pairs       the (u, v) pair of every slot of the neighbour lists (d_nbr_idx int32 [n, maxk], d_nbr_cnt [n]), slot
+ *                         v * maxk + q -> d_pu / d_pv int32 [n * maxk]; an empty slot gives the pair (n, 0), so the reverse CSR
+ *                         is drb_csr_build with n + 1 rows and its last row dropped.
+ * drb_userknn_place       d_r_val[slot of (u, v) in R] = W[u, v] (the value of u in v's list) for the reverse CSR (d_r_ptr,
+ *                         d_r_col; rows u, ascending v).
+ * drb_userknn_scores      pred_mat[u, c] = sum_{v in R(u)} W[u, v] x_vc for each row's user and its candidates (d_cands int64
+ *                         [n_rows, cand_num]), fp64 over ascending v without FMA -> d_scores fp64 [n_rows, cand_num].
+ * drb_userknn_full_scores the same over every item -> d_scores fp64 [n_rows, item_num].  Ranks go through drb_itemknn_topk. */
+size_t drb_gram_image_bytes(int32_t k_rows, int32_t n, int32_t scale);
+int drb_gram_image(const int64_t *d_row_ptr, const int32_t *d_col, const float *d_val, int32_t k_rows, int32_t n, int32_t scale,
+                   void *d_img, void *stream);
+int drb_gram_panel(const void *d_img, int32_t k_rows, int32_t n, int32_t scale, int32_t p0, int32_t rows, double *d_G, void *stream);
+int drb_knn_neighbours_panel(const double *d_G, int32_t n, int32_t j0, int32_t rows, const float *d_ss, int32_t family,
+                             int32_t normalize, float shrink, int32_t maxk, int32_t *d_nbr_idx, float *d_nbr_val, int32_t *d_nbr_cnt,
+                             void *stream);
+int drb_userknn_transpose(const int64_t *d_row_ptr, const int32_t *d_col, const float *d_val, int32_t user_num,
+                          const int64_t *d_t_ptr, const int32_t *d_t_col, float *d_t_val, int32_t *d_order, void *stream);
+int drb_userknn_pairs(const int32_t *d_nbr_idx, const int32_t *d_nbr_cnt, int32_t n, int32_t maxk, int32_t *d_pu, int32_t *d_pv,
+                      void *stream);
+int drb_userknn_place(const int32_t *d_nbr_idx, const float *d_nbr_val, const int32_t *d_nbr_cnt, int32_t n, int32_t maxk,
+                      const int64_t *d_r_ptr, const int32_t *d_r_col, float *d_r_val, void *stream);
+int drb_userknn_scores(const int64_t *d_row_ptr, const int32_t *d_col, const float *d_val, const int64_t *d_r_ptr,
+                       const int32_t *d_r_col, const float *d_r_val, const int64_t *d_users, int64_t n_rows, const int64_t *d_cands,
+                       int32_t cand_num, double *d_scores, void *stream);
+int drb_userknn_full_scores(const int64_t *d_row_ptr, const int32_t *d_col, const float *d_val, const int64_t *d_r_ptr,
+                            const int32_t *d_r_col, const float *d_r_val, int32_t item_num, const int64_t *d_users, int64_t n_rows,
+                            double *d_scores, void *stream);
+
+/* ---- MostPop: daisy/model/PopRecommender.py, csrc/mostpop.cu --------------------------------------------------------------
+ * drb_mostpop_fit         value_counts of the n item ids d_ids (every row, duplicates included) by integer atomics ->
+ *                         d_cnt fp64 [item_num] (item_cnt_ref) and d_score fp64 [item_num] = cnt / (1 + cnt), correctly rounded
+ *                         as numpy's.  *h_bad = the number of ids outside [0, item_num) (not counted).  d_ws:
+ *                         drb_mostpop_workspace_bytes(item_num) bytes.  Synchronises.
+ * drb_mostpop_gather      d_out[k] = d_score[d_cands[k]] for k < total (rank's candidate scores, ranked by drb_itemknn_topk). */
+size_t drb_mostpop_workspace_bytes(int32_t item_num);
+int drb_mostpop_fit(const int64_t *d_ids, int64_t n, int32_t item_num, void *d_ws, double *d_cnt, double *d_score, int64_t *h_bad,
+                    void *stream);
+int drb_mostpop_gather(const double *d_score, const int64_t *d_cands, int64_t total, double *d_out, void *stream);
+
 /* ---- SLiM: daisy/model/SLiMRecommender.py, csrc/slim.cu --------------------------------------------------------------------
  * Item j's ElasticNet fit (:73-84) in Gram form on G = X^T X fp64 [n, n] (drb_ease_gram, reg 0), l1 = alpha elastic U,
  * l2 = alpha (1 - elastic) U:  min_{w >= 0, w_j = 0} 1/2 w^T G w - G[:, j]^T w + l1 sum(w) + 1/2 l2 |w|^2.
