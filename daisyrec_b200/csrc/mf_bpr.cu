@@ -176,6 +176,14 @@ static int ub_users_for(int U, int F, long long batch)
     const long long nbk = ((long long)U + ub - 1) / ub;
     return (nbk <= kUbMaxBuckets && batch + 4 * nbk < (1LL << 31)) ? ub : 0;
 }
+// SGD stages the bucket's user rows (two slots: the current bucket's and the prefetched next one's) next to the accumulator of
+// `ub` users, when both fit kUbStagedSmem (ub (12 F + 4) bytes); wider buckets keep the accumulate-then-sweep user side
+static bool ub_staged(const StepParams &p, int ub)
+{
+    const size_t acc = sizeof(float) * (size_t)ub * p.F + sizeof(unsigned) * ub;
+    const size_t rows = 2 * sizeof(float) * (size_t)ub * p.F;
+    return p.opt == DRB_OPT_SGD && p.gscale == 1.f && p.neg_mult == 1.f && acc + rows <= kUbStagedSmem;
+}
 
 // The bucketed mode's scratch (counters, bucket ranges, user and item norm cache, partitioned triples): library-owned, grow-only,
 // one per device and stream; it depends on the batch, so it cannot live in the workspace.  Its counters are cleared before every
@@ -237,13 +245,11 @@ static int launch_kernel(StepKernel k, StepParams &p, cudaStream_t st, bool keep
         p.ub_users = ub_users_for(p.U, p.F, p.batch);
         DRB_REQUIRE(p.ub_users > 0, "user-bucketed step: %d users in more than %d buckets", p.U, kUbMaxBuckets);
         p.ub_buckets = (p.U + p.ub_users - 1) / p.ub_users;
-        // SGD stages the bucket's user rows (two slots: the current bucket's and the prefetched next one's) next to the
-        // accumulator, when both fit kUbStagedSmem; wider buckets keep the accumulate-then-sweep user side
-        // (accumulator row stride: F staged, F + 1 otherwise; the staged form adds the item regulariser once per occurrence in
-        // phase 1: unscaled gradients, one count per occurrence)
+        // staged form (ub_staged) or accumulate-then-sweep (accumulator row stride: F staged, F + 1 otherwise; the staged form
+        // adds the item regulariser once per occurrence in phase 1: unscaled gradients, one count per occurrence)
         const size_t acc = sizeof(float) * (size_t)p.ub_users * p.F + sizeof(unsigned) * p.ub_users;
         const size_t rows = 2 * sizeof(float) * (size_t)p.ub_users * p.F;
-        const bool staged = p.opt == DRB_OPT_SGD && p.gscale == 1.f && p.neg_mult == 1.f && acc + rows <= kUbStagedSmem;
+        const bool staged = ub_staged(p, p.ub_users);
         const size_t need = staged ? acc + rows : acc + sizeof(float) * (size_t)p.ub_users;
         const size_t hist = 2 * sizeof(unsigned) * (size_t)p.ub_buckets;
         smem = ((need > hist ? need : hist) + 15) / 16 * 16;
@@ -551,14 +557,15 @@ void lean_geom(int F, long long table_rows, int &W, int &NCH)
 }
 int lean_tile_cap(int F, long long table_rows) { return lean_choice(F, table_rows).tile_cap; }
 
-// which instantiation the last launch_steps call of any thread ran: 0 general, 1 lean, 2 lean user-bucketed
-static std::atomic<int> g_last_step_mode{0};
+// which instantiation the last launch_steps call of any thread ran: 0 general, 1 lean, 2 lean user-bucketed; and whether that
+// user-bucketed launch ran the staged SGD form (1) or the accumulate-then-sweep one (0)
+static std::atomic<int> g_last_step_mode{0}, g_last_step_staged{0};
 
 int launch_steps(StepParams &p, cudaStream_t st, bool keep_status)
 {
     // lean: the MF hot path; GEN: any loss but BPR, Adagrad / RMSprop sweeps, FM biases, deterministic accumulation
     StepKernel k = nullptr;
-    int tile_cap = kTileDefault, mode = 0;
+    int tile_cap = kTileDefault, mode = 0, staged = 0;
     bool ub = false;
     if (step_params_lean(p)) {
         const LeanChoice &c = lean_choice(p.F, (long long)p.U + p.I);
@@ -570,6 +577,7 @@ int launch_steps(StepParams &p, cudaStream_t st, bool keep_status)
             tile_cap = c.tile_cap;
             ub = true;
             mode = 2;
+            staged = ub_staged(p, ub_users_for(p.U, p.F, p.batch)) ? 1 : 0;
         } else if (c.W > 0) {
             k = pick_lean_wn(c.W, c.NCH);
             tile_cap = c.tile_cap;
@@ -584,6 +592,7 @@ int launch_steps(StepParams &p, cudaStream_t st, bool keep_status)
                 "workspace from drb_mf_workspace_bytes_det");
     DRB_REQUIRE(k != nullptr, "unsupported factors=%d (row too long for 32 lanes x 8 chunks)", p.F);
     g_last_step_mode = mode;
+    g_last_step_staged = staged;
     return launch_kernel(k, p, st, keep_status, tile_cap, ub);
 }
 
@@ -631,6 +640,10 @@ extern "C" int drb_mf_step_variant(int32_t F, int64_t table_rows, int32_t *lanes
 // which instantiation the last BPR step launch ran: 0 general, 1 lean, 2 lean user-bucketed (a launch-time choice: the bucketed
 // mode also depends on the launch's batch and phases)
 extern "C" int drb_mf_last_step_mode(void) { return drb::g_last_step_mode; }
+
+// 1 when that launch ran the user-bucketed mode in its staged SGD form, 0 otherwise (the form depends on the optimiser and the
+// bucket width)
+extern "C" int drb_mf_last_step_staged(void) { return drb::g_last_step_staged; }
 
 // the timing half of the on-device selection for `factors`: milliseconds of the timed launch (3 steps of 524 288 triples) of the
 // general instantiation and of the best lean candidate, and the index-tile cap in use (runs the selection if it has not run)

@@ -87,6 +87,10 @@ int drb_mf_step_variant(int32_t factors, int64_t table_rows, int32_t *lanes, int
 int drb_mf_step_selfcheck_ms(int32_t factors, int64_t table_rows, float *ms_general, float *ms_lean, int32_t *tile_cap);
 /* Which instantiation the last BPR step launch ran: 0 general, 1 lean, 2 lean user-bucketed. */
 int drb_mf_last_step_mode(void);
+/* Which form of the user-bucketed mode that launch ran: 1 the staged SGD form (each bucket's user rows in shared memory,
+ * updated when the bucket completes), 0 the accumulate-then-sweep form (Adam, or buckets too wide to stage) or no
+ * user-bucketed launch. */
+int drb_mf_last_step_staged(void);
 /* Host-only companion (no device): lane geometry of the lean (lean != 0) or canonical instantiation, and the tile size the
  * launcher picks for `per_cta` triples per CTA and step.  DRB_ERR_INVALID when no instantiation exists for `factors`. */
 int drb_mf_step_geometry(int32_t factors, int32_t lean, int32_t *lanes, int32_t *chunks, int64_t per_cta, int32_t *tile);

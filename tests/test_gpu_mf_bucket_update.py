@@ -43,18 +43,19 @@ for name, (F, U, I, B, n, hot, lr, reg, halve) in cases.items():
     o = (ctypes.c_int64 * 8)()
     L.check(L.lib().drb_mf_workspace_layout(U, I, F, L.OPT_KIND["sgd"], o))
     buf = ws.buf
-    losses, modes, nonzero = [], [], []
+    losses, modes, forms, nonzero = [], [], [], []
     for first, k in ((0, 2), (2, K - 2)):
         if first and halve:
             P.mul_(0.5)                             # the user norms the first launch cached are stale now
         losses.append(ops.mf_bpr_train_steps(P, Q, ws, bu, bi, bj, B, first, k, hp).cpu().numpy())
         modes.append(L.lib().drb_mf_last_step_mode())
+        forms.append(L.lib().drb_mf_last_step_staged())
         torch.cuda.synchronize()
         # gP, gQ, cntU, cntI: zero between launches
         acc = [buf[o[6]:o[6] + 4 * U * F], buf[o[2]:o[2] + o[3]], buf[o[7]:o[7] + 4 * U], buf[o[4]:o[4] + o[5]]]
         nonzero.append(sum(int(a.count_nonzero()) for a in acc))
     np.savez(f"{outdir}/{name}.npz", P=P.cpu().numpy(), Q=Q.cpu().numpy(), loss=np.concatenate(losses), modes=np.array(modes),
-             nonzero=np.array(nonzero))
+             forms=np.array(forms), nonzero=np.array(nonzero))
 """
 
 # name: F, U, I, batch, triples, hot user + empty bucket, lr, reg_1 = reg_2, halve P between the launches.  lr 0.01 with a hot
@@ -96,6 +97,7 @@ def test_bucket_update_matches_general(tmp_path_factory, name):
     got = np.load(out["bucketed"] / f"{name}.npz")
     assert list(ref["modes"]) == [0, 0]
     assert list(got["modes"]) == [2, 2], got["modes"]       # both launches ran the bucketed mode
+    assert list(got["forms"]) == [1, 1] and list(ref["forms"]) == [0, 0], got["forms"]   # in its staged SGD form
     assert np.all(ref["loss"] > 0)
     np.testing.assert_allclose(got["loss"], ref["loss"], rtol=1e-5)
     for t in ("P", "Q"):

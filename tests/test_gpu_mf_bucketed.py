@@ -36,17 +36,18 @@ bu, bi, bj = (torch.from_numpy(x).cuda() for x in (u, i, j))
 ws = ops.MFWorkspace(U, I, F, opt, "cuda")
 hp = ops.hyper(lr, 0.001, 0.001, opt=opt)
 K = (n + B - 1) // B
-losses, modes = [], []                               # modes: the instantiation each launch ran (2 = user-bucketed)
+losses, modes, forms = [], [], []                    # modes: the instantiation each launch ran (2 = user-bucketed)
 for first, k in ((0, 2), (2, K - 2)):
     losses.append(ops.mf_bpr_train_steps(P, Q, ws, bu, bi, bj, B, first, k, hp, adam_step0=first).cpu().numpy())
     modes.append(L.lib().drb_mf_last_step_mode())
+    forms.append(L.lib().drb_mf_last_step_staged())   # 1: staged SGD form
 torch.cuda.synchronize()
 o = (ctypes.c_int64 * 8)()
 L.check(L.lib().drb_mf_workspace_layout(U, I, F, L.OPT_KIND[opt], o))
 buf = ws.buf
 acc = [buf[o[6]:o[6] + 4 * U * F], buf[o[2]:o[2] + o[3]], buf[o[7]:o[7] + 4 * U], buf[o[4]:o[4] + o[5]]]
 np.savez(out, P=P.cpu().numpy(), Q=Q.cpu().numpy(), loss=np.concatenate(losses),
-         variant=L.lib().drb_mf_step_variant(F, U + I, None, None), modes=np.array(modes),
+         variant=L.lib().drb_mf_step_variant(F, U + I, None, None), modes=np.array(modes), forms=np.array(forms),
          acc_nonzero=sum(int(a.count_nonzero()) for a in acc))
 """
 
@@ -92,6 +93,10 @@ def test_bucketed_matches_general(tmp_path, F, opt, U, I, B, n, hot, lr):
         assert list(got["modes"]) == [2, 2], got["modes"]
     else:
         assert 2 not in list(got["modes"]), got["modes"]
+    # at these widths (16 users per bucket) the bucketed mode stages its user rows under SGD, and keeps the
+    # accumulate-then-sweep user side under Adam
+    staged = int(F in (32, 64) and opt == "sgd")
+    assert list(got["forms"]) == [staged, staged] and list(ref["forms"]) == [0, 0], got["forms"]
     np.testing.assert_allclose(got["loss"], ref["loss"], rtol=1e-5)
     assert np.all(ref["loss"] > 0)
     for t in ("P", "Q"):
