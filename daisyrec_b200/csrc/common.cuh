@@ -36,6 +36,9 @@ inline int grid_for(long long n, int block, int per_sm = 16)
     return (int)(b < 1 ? 1 : b);
 }
 
+// threshold of the counter-based keep rule (drop_kept below) for a dropout probability p in [0, 1)
+inline uint32_t drop_thresh(double p) { return (uint32_t)fmin(4294967295.0, p * 4294967296.0); }
+
 // ---------------------------------------------------------------- row geometry
 // A factor row of F floats is processed by a group of W lanes (W a power of two <= 32);
 // lane l owns the chunks c = l, l+W, ... of VEC consecutive floats (NCH chunks per lane at most).
@@ -238,6 +241,19 @@ __device__ __forceinline__ void philox4x32(uint32_t (&c)[4], uint32_t k0, uint32
         k0 += 0x9E3779B9u;
         k1 += 0xBB67AE85u;
     }
+}
+__device__ __forceinline__ uint32_t philox_word(const uint32_t (&c)[4], unsigned k)
+{
+    return k == 0 ? c[0] : k == 1 ? c[1] : k == 2 ? c[2] : c[3];
+}
+
+// ---------------------------------------------------------------- counter-based dropout: the one keep rule
+// An element is kept iff its Philox word >= thresh (drop_thresh(p) = p * 2^32, so P(keep) = 1 - p), and a kept value is
+// scaled by inv_keep.  NeuMF, NGCF and NFM draw their masks with it; each model keys its own counters.
+__device__ __forceinline__ bool drop_kept(uint32_t word, uint32_t thresh) { return word >= thresh; }
+__device__ __forceinline__ float drop_apply(float v, uint32_t word, uint32_t thresh, float inv_keep)
+{
+    return drop_kept(word, thresh) ? v * inv_keep : 0.f;
 }
 
 // ---------------------------------------------------------------- grid-wide barrier

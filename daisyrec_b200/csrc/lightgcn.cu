@@ -65,10 +65,25 @@ static size_t carve_lgcn(void *base, int U, int I, int F, int opt, LgcnWs *w)
 }
 
 
-// Y[r] (+)= sum_e val[e] * X[col[e]]  over the segment's edges;  S[r] += the same (layer-sum accumulator)
-template <int VEC, int W, int NCH>
-__global__ void __launch_bounds__(kSpmmThreads) spmm_seg_kernel(Adj a, const float *__restrict__ X, float *__restrict__ Y,
-                                                                float *__restrict__ S, int F)
+// weight of CSR slot e under node dropout.  DROP 1 walks the slots in order, so one Philox call serves four consecutive slots
+// (`words` caches chunk `wchunk`); DROP 2 reads the keep of the mirror slot, one call per edge.
+template <int DROP>
+__device__ __forceinline__ float edge_weight(const EdgeDrop &ed, long long e, float val, unsigned long long &wchunk,
+                                             uint32_t (&words)[4])
+{
+    const unsigned long long slot = DROP == 2 ? (unsigned long long)__ldg(ed.mirror + e) : (unsigned long long)e;
+    if (DROP == 2 || (slot >> 2) != wchunk) {
+        wchunk = slot >> 2;
+        edge_words(ed, wchunk, words);
+    }
+    return drop_apply(val, philox_word(words, (unsigned)(slot & 3)), ed.thresh, ed.inv_keep);
+}
+
+// Y[r] (+)= sum_e val[e] * X[col[e]]  over the segment's edges;  S[r] += the same (layer-sum accumulator).
+// DROP (NGCF's node dropout, spmm.cuh): 0 none; 1 val[e] -> keep(e) ? val[e] * inv_keep : 0; 2 the same with keep(mirror[e]).
+template <int VEC, int W, int NCH, int DROP>
+__device__ __forceinline__ void spmm_seg_body(const Adj &a, const float *__restrict__ X, float *__restrict__ Y,
+                                              float *__restrict__ S, int F, const EdgeDrop &ed)
 {
     constexpr int GPW = 32 / W, GROUPS = (kSpmmThreads / 32) * GPW, E = 4;
     const int lane = threadIdx.x & 31, gl = lane % W;
@@ -82,6 +97,8 @@ __global__ void __launch_bounds__(kSpmmThreads) spmm_seg_kernel(Adj a, const flo
         for (int ch = 0; ch < NCH; ++ch)
 #pragma unroll
             for (int q = 0; q < VEC; ++q) acc.c[ch].v[q] = 0.f;
+        unsigned long long wchunk = ~0ull;     // DROP == 1: the slot chunk whose Philox words are in `words`
+        uint32_t words[4];
         // main loop: whole groups of E edges, no bounds checks (a full segment is 256 edges = 64 iterations)
         long long e0 = b;
         for (; e0 + E <= e; e0 += E) {
@@ -91,6 +108,7 @@ __global__ void __launch_bounds__(kSpmmThreads) spmm_seg_kernel(Adj a, const flo
             for (int q = 0; q < E; ++q) {
                 const int cq = __ldg(a.col + e0 + q);
                 vv[q] = __ldg(a.val + e0 + q);
+                if constexpr (DROP != 0) vv[q] = edge_weight<DROP>(ed, e0 + q, vv[q], wchunk, words);
                 x[q] = load_row<VEC, W, NCH>(X + (size_t)cq * F, gl, chunks, true);
             }
 #pragma unroll
@@ -103,7 +121,8 @@ __global__ void __launch_bounds__(kSpmmThreads) spmm_seg_kernel(Adj a, const flo
         // tail: fewer than E edges left, same ascending-column accumulation order
         for (; e0 < e; ++e0) {
             const int cq = __ldg(a.col + e0);
-            const float v1 = __ldg(a.val + e0);
+            float v1 = __ldg(a.val + e0);
+            if constexpr (DROP != 0) v1 = edge_weight<DROP>(ed, e0, v1, wchunk, words);
             const Row<VEC, W, NCH> x1 = load_row<VEC, W, NCH>(X + (size_t)cq * F, gl, chunks, true);
 #pragma unroll
             for (int ch = 0; ch < NCH; ++ch)
@@ -130,6 +149,20 @@ __global__ void __launch_bounds__(kSpmmThreads) spmm_seg_kernel(Adj a, const flo
             }
         }
     }
+}
+
+template <int VEC, int W, int NCH>
+__global__ void __launch_bounds__(kSpmmThreads) spmm_seg_kernel(Adj a, const float *__restrict__ X, float *__restrict__ Y,
+                                                                float *__restrict__ S, int F)
+{
+    spmm_seg_body<VEC, W, NCH, 0>(a, X, Y, S, F, EdgeDrop{});
+}
+
+template <int VEC, int W, int NCH, int DROP>
+__global__ void __launch_bounds__(kSpmmThreads) spmm_seg_drop_kernel(Adj a, const float *__restrict__ X, float *__restrict__ Y,
+                                                                     int F, EdgeDrop ed)
+{
+    spmm_seg_body<VEC, W, NCH, DROP>(a, X, Y, nullptr, F, ed);
 }
 
 __global__ void scale_kernel(float *__restrict__ x, long long n4, float s)
@@ -169,6 +202,37 @@ int launch_spmm(const Adj &a, const float *X, float *Y, float *S, int F, cudaStr
     if (a.nseg == 0) return DRB_OK;
     const int groups = (kSpmmThreads / 32) * (32 / g.width);
     k<<<grid_for(a.nseg, groups, 8), kSpmmThreads, 0, st>>>(a, X, Y, S, F);
+    DRB_CUDA(cudaGetLastError());
+    return DRB_OK;
+}
+
+typedef void (*SpmmDropKernel)(Adj, const float *, float *, int, EdgeDrop);
+template <int VEC, int DROP>
+static SpmmDropKernel pick_spmm_drop_v(int W, int NCH)
+{
+#define DRB_CASE(w, n) \
+    if (W == w && NCH == n) return spmm_seg_drop_kernel<VEC, w, n, DROP>;
+    DRB_CASE(1, 1) DRB_CASE(2, 1) DRB_CASE(4, 1) DRB_CASE(8, 1) DRB_CASE(16, 1) DRB_CASE(32, 1)
+    DRB_CASE(32, 2) DRB_CASE(32, 4) DRB_CASE(32, 8)
+#undef DRB_CASE
+    return nullptr;
+}
+template <int DROP>
+static SpmmDropKernel pick_spmm_drop(const RowGeom &g)
+{
+    return g.vec == 4 ? pick_spmm_drop_v<4, DROP>(g.width, g.nch) : g.vec == 2 ? pick_spmm_drop_v<2, DROP>(g.width, g.nch)
+                                                                               : pick_spmm_drop_v<1, DROP>(g.width, g.nch);
+}
+
+int launch_spmm_drop(const Adj &a, const float *X, float *Y, int F, const EdgeDrop &ed, cudaStream_t st)
+{
+    RowGeom g = row_geom(F);
+    SpmmDropKernel k = ed.mirror ? pick_spmm_drop<2>(g) : pick_spmm_drop<1>(g);
+    DRB_REQUIRE(k != nullptr, "unsupported factors=%d", F);
+    DRB_CUDA(cudaMemsetAsync(Y, 0, sizeof(float) * (size_t)a.n * F, st));
+    if (a.nseg == 0) return DRB_OK;
+    const int groups = (kSpmmThreads / 32) * (32 / g.width);
+    k<<<grid_for(a.nseg, groups, 8), kSpmmThreads, 0, st>>>(a, X, Y, F, ed);
     DRB_CUDA(cudaGetLastError());
     return DRB_OK;
 }

@@ -215,7 +215,7 @@ static int launch_gemm(int dtype, long long M, int N, int K, const float *A, lon
 // ------------------------------------------------------------------------------------------ gather / head / scatter
 // Dropout (NeuMFRecommender.py:61: nn.Dropout in front of every Linear, active in train mode).  The reference draws its
 // masks from torch's global RNG; here they are counter-based: keep(layer, step, element) = Philox4x32-10(seed;
-// element/4, layer, step) word (element%4) >= p * 2^32.  Counter-based masks can be regenerated in the backward pass
+// element/4, layer, step) word (element%4) >= p * 2^32 (drop_kept, common.cuh).  Counter-based masks can be regenerated in the backward pass
 // (layer 0) instead of being stored.  Kept values are scaled by 1/(1-p) like torch.
 // Parity mode: `bits[layer]` points at HOST-generated keep masks for this step -- the very tensors
 // torch.empty(B, n_l).bernoulli_(1 - p) yields on the CPU generator, in the reference's draw order, bit-packed (bit e of
@@ -238,10 +238,10 @@ __device__ __forceinline__ float4 drop4(float4 v, const Drop &d, unsigned long l
     }
     uint32_t c[4] = {(uint32_t)chunk, (uint32_t)(chunk >> 32), layer, d.step};
     philox4x32(c, d.k0, d.k1);
-    v.x = c[0] >= d.thresh ? v.x * d.inv_keep : 0.f;
-    v.y = c[1] >= d.thresh ? v.y * d.inv_keep : 0.f;
-    v.z = c[2] >= d.thresh ? v.z * d.inv_keep : 0.f;
-    v.w = c[3] >= d.thresh ? v.w * d.inv_keep : 0.f;
+    v.x = drop_apply(v.x, c[0], d.thresh, d.inv_keep);
+    v.y = drop_apply(v.y, c[1], d.thresh, d.inv_keep);
+    v.z = drop_apply(v.z, c[2], d.thresh, d.inv_keep);
+    v.w = drop_apply(v.w, c[3], d.thresh, d.inv_keep);
     return v;
 }
 
@@ -728,7 +728,7 @@ extern "C" int drb_neumf_bpr_train_steps(float *d_UG, float *d_IG, float *d_UM, 
         drop.p = dropout; drop.inv_keep = 1.f / (1.f - dropout);
         drop.k0 = (uint32_t)dropout_seed; drop.k1 = (uint32_t)(dropout_seed >> 32);
         drop.step = (uint32_t)(adam_step0 + s);
-        drop.thresh = (uint32_t)fmin(4294967295.0, (double)dropout * 4294967296.0);
+        drop.thresh = drop_thresh((double)dropout);
         for (int l = 0; l < kMaxLayers; ++l) drop.bits[l] = nullptr;
         if (d_drop_masks && dropout > 0.f) {                  // parity mode: this step's host-generated masks, per layer
             DRB_REQUIRE(B == batch, "neumf: host dropout masks need full batches (n must be a multiple of batch)");

@@ -235,19 +235,44 @@ __global__ void nfm_act_kernel(const float *__restrict__ z, long long total, int
 
 // nn.Dropout with the caller's masks (NFMRecommender.py:67,:88): x *= keep ? 1/(1-p) : 0, in place.  keep is laid out as torch
 // drew it: [forward call (pos, neg)][site][B][F] bytes; rows [0,B) belong to the positive call, [B,2B) to the negative one.
-__device__ __forceinline__ float nfm_keep_factor(const uint8_t *__restrict__ keep, long long k, long long B, int F, int site,
-                                                 int nsites, float scale)
+// keep == nullptr: the masks come from Philox on the device (dropout_engine 'philox'), keyed by (seed, global step, forward call,
+// site, row, column chunk) through the common keep rule: element (t, f) of a call is kept iff word f % 4 of
+// Philox4x32-10(seed; f / 4, t, site | call << 8, step) >= p * 2^32.
+struct NfmDrop {
+    uint32_t k0, k1, step, thresh;
+};
+__device__ __forceinline__ float nfm_keep_factor(const uint8_t *__restrict__ keep, const NfmDrop &nd, long long k, long long B,
+                                                 int F, int site, int nsites, float scale)
 {
     const long long r = k / F;
     const int f = (int)(k - r * F);
     const long long pass = r >= B ? 1 : 0, t = r - pass * B;
-    return keep[((pass * nsites + site) * B + t) * F + f] ? scale : 0.f;
+    if (keep) return keep[((pass * nsites + site) * B + t) * F + f] ? scale : 0.f;
+    uint32_t c[4] = {(uint32_t)f >> 2, (uint32_t)t, (uint32_t)site | ((uint32_t)pass << 8), nd.step};
+    philox4x32(c, nd.k0, nd.k1);
+    return drop_kept(philox_word(c, (unsigned)f & 3u), nd.thresh) ? scale : 0.f;
 }
-__global__ void nfm_dropout_kernel(float *__restrict__ x, const uint8_t *__restrict__ keep, long long B, long long total, int F,
-                                   int site, int nsites, float scale)
+__global__ void nfm_dropout_kernel(float *__restrict__ x, const uint8_t *__restrict__ keep, NfmDrop nd, long long B, long long total,
+                                   int F, int site, int nsites, float scale)
 {
     for (long long k = (long long)blockIdx.x * blockDim.x + threadIdx.x; k < total; k += (long long)gridDim.x * blockDim.x)
-        x[k] = x[k] * nfm_keep_factor(keep, k, B, F, site, nsites, scale);
+        x[k] = x[k] * nfm_keep_factor(keep, nd, k, B, F, site, nsites, scale);
+}
+// test hook: one step's Philox masks as bytes in the layout of keep ([call][site][B][F]), through nfm_keep_factor
+__global__ void nfm_philox_masks_kernel(NfmDrop nd, long long B, int F, int nsites, uint8_t *__restrict__ out)
+{
+    const long long total = 2 * nsites * B * F;
+    for (long long k = (long long)blockIdx.x * blockDim.x + threadIdx.x; k < total; k += (long long)gridDim.x * blockDim.x) {
+        const long long per = B * F, blk = k / per, rem = k - blk * per;
+        const int pass = (int)(blk / nsites), site = (int)(blk - (long long)pass * nsites);
+        out[k] = nfm_keep_factor(nullptr, nd, pass * per + rem, B, F, site, nsites, 1.f) != 0.f ? 1 : 0;
+    }
+}
+static NfmDrop make_nfm_drop(uint64_t seed, int64_t step, float p)
+{
+    NfmDrop d;
+    d.k0 = (uint32_t)seed; d.k1 = (uint32_t)(seed >> 32); d.step = (uint32_t)step; d.thresh = drop_thresh((double)p);
+    return d;
 }
 
 // one warp per row: fm = h + ((u_bias + i_bias) + bias_), pred = <fm, wp>   (rows given by (bu, bi|bj) or by explicit pairs)
@@ -396,12 +421,12 @@ __global__ void nfm_act_bwd_kernel(const float *__restrict__ dh, const float *__
 }
 // the same behind a Dropout: tmp = (dh * keep factor) * act'(z, act(z))  (h holds the dropped activations, so act(z) is redone)
 __global__ void nfm_act_bwd_drop_kernel(const float *__restrict__ dh, const float *__restrict__ z, const uint8_t *__restrict__ keep,
-                                        long long B, long long total, int F, int site, int nsites, float scale, int act,
+                                        NfmDrop nd, long long B, long long total, int F, int site, int nsites, float scale, int act,
                                         float *__restrict__ out)
 {
     for (long long k = (long long)blockIdx.x * blockDim.x + threadIdx.x; k < total; k += (long long)gridDim.x * blockDim.x) {
         const float zz = z[k];
-        out[k] = (dh[k] * nfm_keep_factor(keep, k, B, F, site, nsites, scale)) * nfm_act_grad(act, zz, nfm_act(act, zz));
+        out[k] = (dh[k] * nfm_keep_factor(keep, nd, k, B, F, site, nsites, scale)) * nfm_act_grad(act, zz, nfm_act(act, zz));
     }
 }
 
@@ -515,19 +540,17 @@ extern "C" int drb_nfm_workspace_init(void *d_ws, int32_t U, int32_t I, int32_t 
 // for the n_steps steps in order: per step [forward call: pos, neg][site: FM_layers' Dropout, then the one behind each
 // activation][batch][F] (the caller draws them on torch's CPU generator in exactly that order; a ragged last batch uses its own
 // row count).  Every step must hold `batch` triples when n_steps > 1.  d_keep = NULL: no dropout.
-extern "C" int drb_nfm_bpr_train_steps(float *d_P, float *d_Q, float *d_bias, float *d_N, float *d_Rs, void *d_ws, int32_t U,
-                                       int32_t I, int32_t F, int32_t L, int32_t batch_norm, int32_t act, int64_t max_rows,
-                                       const int32_t *d_bu, const int32_t *d_bi, const int32_t *d_bj, int64_t n, int64_t batch,
-                                       int64_t first_step, int64_t n_steps, const drb_hyper *h, int64_t adam_step0, int32_t apply,
-                                       int32_t tower_dtype, const uint8_t *d_keep, float dropout, double *d_step_loss,
-                                       int32_t sync_and_check, int64_t *nan_step, void *stream)
+// philox: the masks come from Philox keyed by (seed, adam_step0 + s) instead of d_keep (dropout > 0: on).
+static int nfm_train(float *d_P, float *d_Q, float *d_bias, float *d_N, float *d_Rs, void *d_ws, int32_t U, int32_t I, int32_t F,
+                     int32_t L, int32_t batch_norm, int32_t act, int64_t max_rows, const int32_t *d_bu, const int32_t *d_bi,
+                     const int32_t *d_bj, int64_t n, int64_t batch, int64_t first_step, int64_t n_steps, const drb_hyper *h,
+                     int64_t adam_step0, int32_t apply, int32_t tower_dtype, const uint8_t *d_keep, float dropout, bool philox,
+                     uint64_t seed, double *d_step_loss, int32_t sync_and_check, int64_t *nan_step, void *stream)
 {
     NfmDims d;
-    DRB_REQUIRE(d_keep == nullptr || (dropout > 0.f && dropout < 1.f), "nfm: dropout masks need 0 < dropout < 1");
-    DRB_REQUIRE(d_keep == nullptr || n_steps <= 1 || (first_step + n_steps) * batch <= n,
-                "nfm: with dropout masks every step of a multi-step call must be a full batch");
     const int nsites = 1 + L;
-    const float drop_scale = d_keep ? 1.0f / (float)(1.0 - (double)dropout) : 1.f;
+    const bool drop = d_keep != nullptr || (philox && dropout > 0.f);
+    const float drop_scale = drop ? 1.0f / (float)(1.0 - (double)dropout) : 1.f;
     DRB_REQUIRE(d_P && d_Q && d_bias && d_N && d_ws && d_bu && d_bi && d_bj && h && d_step_loss, "nfm_train_steps: null argument");
     DRB_REQUIRE(nfm_dims(d, U, I, F, L, batch_norm, act), "nfm_train_steps: bad dims (factors <= 256, 0 <= num_layers <= 8, act 0..2)");
     DRB_REQUIRE(!batch_norm || d_Rs, "nfm_train_steps: batch_norm needs the running-statistics block");
@@ -552,6 +575,7 @@ extern "C" int drb_nfm_bpr_train_steps(float *d_P, float *d_Q, float *d_bias, fl
         const long long R = 2 * B, tot = R * F;
         const int32_t *bu = d_bu + base, *bi = d_bi + base, *bj = d_bj + base;
         const uint8_t *keep = d_keep ? d_keep + (size_t)s * 2 * nsites * (size_t)batch * F : nullptr;   // this step's masks
+        const NfmDrop nd = make_nfm_drop(seed, adam_step0 + s, dropout);
         int rc = DRB_OK;
         // ---- forward (both calls at once; BatchNorm statistics per half)
         nfm_product_kernel<<<grid_for(tot, 256), 256, 0, st>>>(d_P, d_Q, bu, bi, bj, B, R, F, w.e);
@@ -562,8 +586,8 @@ extern "C" int drb_nfm_bpr_train_steps(float *d_P, float *d_Q, float *d_bias, fl
             if (rc != DRB_OK) return rc;
             h_fm = w.h0;
         }
-        if (keep) {
-            nfm_dropout_kernel<<<grid_for(tot, 256), 256, 0, st>>>(h_fm, keep, B, tot, F, 0, nsites, drop_scale);
+        if (drop) {
+            nfm_dropout_kernel<<<grid_for(tot, 256), 256, 0, st>>>(h_fm, keep, nd, B, tot, F, 0, nsites, drop_scale);
             DRB_CUDA(cudaGetLastError());
         }
         const float *hin = h_fm;
@@ -580,8 +604,8 @@ extern "C" int drb_nfm_bpr_train_steps(float *d_P, float *d_Q, float *d_bias, fl
             }
             nfm_act_kernel<<<grid_for(tot, 256), 256, 0, st>>>(w.z[l], tot, d.act, w.h[l]);
             DRB_CUDA(cudaGetLastError());
-            if (keep) {
-                nfm_dropout_kernel<<<grid_for(tot, 256), 256, 0, st>>>(w.h[l], keep, B, tot, F, 1 + l, nsites, drop_scale);
+            if (drop) {
+                nfm_dropout_kernel<<<grid_for(tot, 256), 256, 0, st>>>(w.h[l], keep, nd, B, tot, F, 1 + l, nsites, drop_scale);
                 DRB_CUDA(cudaGetLastError());
             }
             hin = w.h[l];
@@ -601,9 +625,9 @@ extern "C" int drb_nfm_bpr_train_steps(float *d_P, float *d_Q, float *d_bias, fl
             const float *W = d_N + d.oW[l];
             const float *hprev = l == 0 ? (d.bn ? w.h0 : w.e) : w.h[l - 1];
             float *gW = w.gN + d.oW[l], *gb = gW + (size_t)F * F;
-            if (keep)
-                nfm_act_bwd_drop_kernel<<<grid_for(tot, 256), 256, 0, st>>>(w.dh, w.z[l], keep, B, tot, F, 1 + l, nsites, drop_scale,
-                                                                          d.act, w.tmp);
+            if (drop)
+                nfm_act_bwd_drop_kernel<<<grid_for(tot, 256), 256, 0, st>>>(w.dh, w.z[l], keep, nd, B, tot, F, 1 + l, nsites,
+                                                                          drop_scale, d.act, w.tmp);
             else
                 nfm_act_bwd_kernel<<<grid_for(tot, 256), 256, 0, st>>>(w.dh, w.z[l], w.h[l], tot, d.act, w.tmp);   // d act input
             DRB_CUDA(cudaGetLastError());
@@ -620,8 +644,8 @@ extern "C" int drb_nfm_bpr_train_steps(float *d_P, float *d_Q, float *d_bias, fl
             if (rc != DRB_OK) return rc;
             if (dprev != w.dh) DRB_CUDA(cudaMemcpyAsync(w.dh, dprev, sizeof(float) * (size_t)tot, cudaMemcpyDeviceToDevice, st));
         }
-        if (keep) {                                                       // backward of FM_layers' Dropout
-            nfm_dropout_kernel<<<grid_for(tot, 256), 256, 0, st>>>(w.dh, keep, B, tot, F, 0, nsites, drop_scale);
+        if (drop) {                                                       // backward of FM_layers' Dropout
+            nfm_dropout_kernel<<<grid_for(tot, 256), 256, 0, st>>>(w.dh, keep, nd, B, tot, F, 0, nsites, drop_scale);
             DRB_CUDA(cudaGetLastError());
         }
         if (d.bn) {
@@ -644,6 +668,49 @@ extern "C" int drb_nfm_bpr_train_steps(float *d_P, float *d_Q, float *d_bias, fl
         if (rc != DRB_OK) return rc;
     }
     if (sync_and_check) return check_nan(d_ws, st, nan_step);
+    return DRB_OK;
+}
+
+extern "C" int drb_nfm_bpr_train_steps(float *d_P, float *d_Q, float *d_bias, float *d_N, float *d_Rs, void *d_ws, int32_t U,
+                                       int32_t I, int32_t F, int32_t L, int32_t batch_norm, int32_t act, int64_t max_rows,
+                                       const int32_t *d_bu, const int32_t *d_bi, const int32_t *d_bj, int64_t n, int64_t batch,
+                                       int64_t first_step, int64_t n_steps, const drb_hyper *h, int64_t adam_step0, int32_t apply,
+                                       int32_t tower_dtype, const uint8_t *d_keep, float dropout, double *d_step_loss,
+                                       int32_t sync_and_check, int64_t *nan_step, void *stream)
+{
+    DRB_REQUIRE(d_keep == nullptr || (dropout > 0.f && dropout < 1.f), "nfm: dropout masks need 0 < dropout < 1");
+    DRB_REQUIRE(d_keep == nullptr || n_steps <= 1 || (first_step + n_steps) * batch <= n,
+                "nfm: with dropout masks every step of a multi-step call must be a full batch");
+    return nfm_train(d_P, d_Q, d_bias, d_N, d_Rs, d_ws, U, I, F, L, batch_norm, act, max_rows, d_bu, d_bi, d_bj, n, batch, first_step,
+                     n_steps, h, adam_step0, apply, tower_dtype, d_keep, d_keep ? dropout : 0.f, false, 0, d_step_loss,
+                     sync_and_check, nan_step, stream);
+}
+
+// The same steps with the Dropout masks drawn on the device (dropout_engine 'philox'): step s is keyed by (seed, adam_step0 + s);
+// its pos and neg forward calls draw independent masks.  dropout = 0: no dropout.  Ragged last batches are fine.
+extern "C" int drb_nfm_bpr_train_steps_philox(float *d_P, float *d_Q, float *d_bias, float *d_N, float *d_Rs, void *d_ws,
+                                              int32_t U, int32_t I, int32_t F, int32_t L, int32_t batch_norm, int32_t act,
+                                              int64_t max_rows, const int32_t *d_bu, const int32_t *d_bi, const int32_t *d_bj,
+                                              int64_t n, int64_t batch, int64_t first_step, int64_t n_steps, const drb_hyper *h,
+                                              int64_t adam_step0, int32_t apply, int32_t tower_dtype, float dropout, uint64_t seed,
+                                              double *d_step_loss, int32_t sync_and_check, int64_t *nan_step, void *stream)
+{
+    DRB_REQUIRE(dropout >= 0.f && dropout < 1.f, "nfm: dropout must be in [0, 1)");
+    return nfm_train(d_P, d_Q, d_bias, d_N, d_Rs, d_ws, U, I, F, L, batch_norm, act, max_rows, d_bu, d_bi, d_bj, n, batch, first_step,
+                     n_steps, h, adam_step0, apply, tower_dtype, nullptr, dropout, true, seed, d_step_loss, sync_and_check,
+                     nan_step, stream);
+}
+
+// test hook: the Philox masks of step `step` for batches of `rows` triples, uint8 [call: pos, neg][site][rows][factors]
+extern "C" int drb_nfm_philox_masks(uint64_t seed, int64_t step, int64_t rows, int32_t F, int32_t L, float dropout, uint8_t *d_keep,
+                                    void *stream)
+{
+    DRB_REQUIRE(d_keep && rows > 0 && F > 0 && L >= 0 && L <= kNfmMaxL && dropout >= 0.f && dropout < 1.f,
+                "nfm_philox_masks: bad arguments");
+    const long long total = 2LL * (1 + L) * rows * F;
+    nfm_philox_masks_kernel<<<grid_for(total, 256), 256, 0, (cudaStream_t)stream>>>(make_nfm_drop(seed, step, dropout), rows, F,
+                                                                                   1 + L, d_keep);
+    DRB_CUDA(cudaGetLastError());
     return DRB_OK;
 }
 

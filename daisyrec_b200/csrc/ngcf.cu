@@ -108,6 +108,42 @@ static size_t carve_ngcf(void *base, const NgcfDims &q, int opt, NgcfWs *w)
     return off;
 }
 
+// Message dropout on the device (dropout_engine 'philox'): the mask of layer l's [n, d] output is keyed by (seed, forward
+// counter, layer, row, column chunk) through the common keep rule (common.cuh): element (r, o) is kept iff word o % 4 of
+// Philox4x32-10(seed; o / 4, r, l, forward) >= p * 2^32.  The backward regenerates it instead of storing it.
+struct MsgDrop {
+    uint32_t k0, k1, fwd, thresh;
+    int on;
+};
+static MsgDrop make_msg_drop(uint64_t seed, int64_t fwd, float p)
+{
+    MsgDrop m;
+    m.k0 = (uint32_t)seed; m.k1 = (uint32_t)(seed >> 32); m.fwd = (uint32_t)fwd; m.thresh = drop_thresh((double)p);
+    m.on = p > 0.f;
+    return m;
+}
+static EdgeDrop make_edge_drop(uint64_t seed, int64_t fwd, double p, const int32_t *mirror)
+{
+    EdgeDrop e;
+    e.mirror = mirror; e.k0 = (uint32_t)seed; e.k1 = (uint32_t)(seed >> 32); e.fwd = (uint32_t)fwd;
+    e.thresh = drop_thresh(p);
+    e.inv_keep = (float)(1.0 / (1.0 - p));   // SparseDropout: values * (1.0 / kprob) on an fp32 tensor
+    return e;
+}
+__device__ __forceinline__ bool ngcf_msg_kept(const MsgDrop &m, int layer, long long r, int o)
+{
+    uint32_t c[4] = {(uint32_t)o >> 2, (uint32_t)r, (uint32_t)layer, m.fwd};
+    philox4x32(c, m.k0, m.k1);
+    return drop_kept(philox_word(c, (unsigned)o & 3u), m.thresh);
+}
+// the dropout factor of element (r, o): the host mask's byte when given, else the Philox mask's (1 when neither is on)
+__device__ __forceinline__ float ngcf_drop_factor(const uint8_t *__restrict__ keep, const MsgDrop &m, int layer, long long r,
+                                                  int d, int o, float scale)
+{
+    if (keep) return keep[r * d + o] ? scale : 0.f;
+    return ngcf_msg_kept(m, layer, r, o) ? scale : 0.f;
+}
+
 // scalar forms of the two mix kernels for layer widths that are not multiples of 4
 __global__ void ngcf_mix_scalar_kernel(const float *__restrict__ E, const float *__restrict__ X, long long n, int d,
                                        float *__restrict__ ST)
@@ -148,13 +184,15 @@ __global__ void ngcf_mix_kernel(const float *__restrict__ E, const float *__rest
 }
 
 // one warp per row: y = (Y1 + b1) + (Y2 + b2) (:59), z = LeakyReLU_0.2(y), rn = max(||z||_2, 1e-12), N = z / rn (F.normalize :165)
-// keep (optional): the mask nn.Dropout(mess_dropout) draws over this layer's [n, d] output (:164), bytes; z *= keep ? scale : 0
+// keep (optional): the mask nn.Dropout(mess_dropout) draws over this layer's [n, d] output (:164), bytes; z *= keep ? scale : 0.
+// Without bytes and with md.on the mask of layer `layer` comes from Philox (ngcf_msg_kept).
 __global__ void __launch_bounds__(256) ngcf_act_kernel(const float *__restrict__ Y1, const float *__restrict__ Y2,
                                                        const float *__restrict__ b1, const float *__restrict__ b2, long long n,
                                                        int d, float *__restrict__ Y, float *__restrict__ rn, float *__restrict__ N,
                                                        float *__restrict__ ALL, int C, int coff, const uint8_t *__restrict__ keep,
-                                                       float scale)
+                                                       float scale, MsgDrop md, int layer)
 {
+    const bool drop = keep != nullptr || md.on;
     const int lane = threadIdx.x & 31;
     const long long warp = ((long long)blockIdx.x * blockDim.x + threadIdx.x) >> 5, nw = ((long long)gridDim.x * blockDim.x) >> 5;
     for (long long r = warp; r < n; r += nw) {
@@ -162,7 +200,7 @@ __global__ void __launch_bounds__(256) ngcf_act_kernel(const float *__restrict__
         for (int o = lane; o < d; o += 32) {
             const float y = (Y1[r * d + o] + b1[o]) + (Y2[r * d + o] + b2[o]);
             float z = y > 0.f ? y : 0.2f * y;
-            if (keep) z = z * (keep[r * d + o] ? scale : 0.f);
+            if (drop) z = z * ngcf_drop_factor(keep, md, layer, r, d, o, scale);
             Y[r * d + o] = y;
             ss += (double)(z * z);
         }
@@ -173,7 +211,7 @@ __global__ void __launch_bounds__(256) ngcf_act_kernel(const float *__restrict__
         for (int o = lane; o < d; o += 32) {
             const float y = Y[r * d + o];
             float z = y > 0.f ? y : 0.2f * y;
-            if (keep) z = z * (keep[r * d + o] ? scale : 0.f);
+            if (drop) z = z * ngcf_drop_factor(keep, md, layer, r, d, o, scale);
             const float v = (float)((double)z / nr);
             N[r * d + o] = v;
             ALL[r * C + coff + o] = v;
@@ -197,8 +235,9 @@ __global__ void __launch_bounds__(256) ngcf_act_bwd_kernel(const float *__restri
                                                            const float *__restrict__ dE, const float *__restrict__ N,
                                                            const float *__restrict__ Y, const float *__restrict__ rn,
                                                            long long n, int d, float *__restrict__ dY,
-                                                           const uint8_t *__restrict__ keep, float scale)
+                                                           const uint8_t *__restrict__ keep, float scale, MsgDrop md, int layer)
 {
+    const bool drop = keep != nullptr || md.on;
     const int lane = threadIdx.x & 31;
     const long long warp = ((long long)blockIdx.x * blockDim.x + threadIdx.x) >> 5, nw = ((long long)gridDim.x * blockDim.x) >> 5;
     for (long long r = warp; r < n; r += nw) {
@@ -213,7 +252,7 @@ __global__ void __launch_bounds__(256) ngcf_act_bwd_kernel(const float *__restri
             const double dn = (double)G[r * C + coff + o] + (dE ? (double)dE[r * d + o] : 0.0);
             const double dz = (nr > 1e-12) ? (dn - (double)N[r * d + o] * dot) / nr : dn / nr;
             float dzf = (float)dz;
-            if (keep) dzf = dzf * (keep[r * d + o] ? scale : 0.f);        // Dropout backward
+            if (drop) dzf = dzf * ngcf_drop_factor(keep, md, layer, r, d, o, scale);   // Dropout backward
             dY[r * d + o] = dzf * (Y[r * d + o] > 0.f ? 1.f : 0.2f);
         }
     }
@@ -286,9 +325,10 @@ __global__ void ngcf_finalize_kernel(WsHeader *hdr, float reg1, float reg2, doub
     if (isnan(loss)) { hdr->status = DRB_ERR_NAN_LOSS; hdr->nan_step = step; }
 }
 
-// keep: masks of the L layers concatenated ([n, d[1]], [n, d[2]], ...), or nullptr
+// keep: masks of the L layers concatenated ([n, d[1]], [n, d[2]], ...), or nullptr; md: the Philox message masks (used when
+// keep == nullptr and md.on); ed: node dropout of A (nullptr: none), one edge mask for every layer of this forward
 static int ngcf_forward(const NgcfDims &q, const NgcfWs &w, const Adj &adj, const float *E0, const float *W, int dtype,
-                        cudaStream_t st, const uint8_t *keep = nullptr, float scale = 1.f)
+                        cudaStream_t st, const uint8_t *keep, float scale, const MsgDrop &md, const EdgeDrop *ed)
 {
     const long long n = q.n;
     ngcf_copy_block_kernel<<<grid_for(n * q.d[0], 256), 256, 0, st>>>(E0, n, q.d[0], w.ALL, q.C, 0);
@@ -297,7 +337,7 @@ static int ngcf_forward(const NgcfDims &q, const NgcfWs &w, const Adj &adj, cons
     for (int l = 0; l < q.L; ++l) {
         const int in = q.d[l], out = q.d[l + 1];
         const float *W1 = W + q.w_off[l], *b1 = W1 + (size_t)in * out, *W2 = b1 + out, *b2 = W2 + (size_t)in * out;
-        int rc = launch_spmm(adj, E, w.X[l], nullptr, in, st);
+        int rc = ed ? launch_spmm_drop(adj, E, w.X[l], in, *ed, st) : launch_spmm(adj, E, w.X[l], nullptr, in, st);
         if (rc != DRB_OK) return rc;
         if (in % 4 == 0) ngcf_mix_kernel<<<grid_for(n * (in / 4), 256), 256, 0, st>>>(E, w.X[l], n, in, w.ST);
         else ngcf_mix_scalar_kernel<<<grid_for(n * in, 256), 256, 0, st>>>(E, w.X[l], n, in, w.ST);
@@ -306,12 +346,80 @@ static int ngcf_forward(const NgcfDims &q, const NgcfWs &w, const Adj &adj, cons
         if (rc == DRB_OK) rc = gemm_nt(dtype, n, out, in, w.ST + in, 2 * in, W2, in, w.Y2, out, st);
         if (rc != DRB_OK) return rc;
         ngcf_act_kernel<<<grid_for(n * 32, 256), 256, 0, st>>>(w.Y1, w.Y2, b1, b2, n, out, w.Y[l], w.rn[l], w.E[l + 1], w.ALL,
-                                                             q.C, q.off[l + 1], keep, scale);
+                                                             q.C, q.off[l + 1], keep, scale, md, l);
         DRB_CUDA(cudaGetLastError());
         if (keep) keep += (size_t)n * out;
         E = w.E[l + 1];
     }
     return DRB_OK;
+}
+
+static int ngcf_forward_call(const float *d_E0, const float *d_W, void *d_ws, int32_t U, int32_t I, const int32_t *dims, int32_t L,
+                             const Adj &adj_in, int32_t tower_dtype, const uint8_t *d_keep, float scale, const MsgDrop &md,
+                             const EdgeDrop *ed, float *d_out, cudaStream_t st)
+{
+    NgcfDims q;
+    DRB_REQUIRE(d_E0 && d_W && d_ws && adj_in.row_ptr && d_out && ngcf_dims(q, U, I, dims, L), "ngcf_forward: bad arguments");
+    NgcfWs w;
+    carve_ngcf(d_ws, q, DRB_OPT_SGD, &w);
+    Adj adj = adj_in;
+    adj.n = q.n;
+    int rc = ngcf_forward(q, w, adj, d_E0, d_W, tower_dtype, st, d_keep, scale, md, ed);
+    if (rc != DRB_OK) return rc;
+    DRB_CUDA(cudaMemcpyAsync(d_out, w.ALL, sizeof(float) * (size_t)q.n * q.C, cudaMemcpyDeviceToDevice, st));
+    return DRB_OK;
+}
+
+static Adj make_adj(const int64_t *d_row_ptr, const int32_t *d_col, const float *d_val, const int32_t *d_seg_row,
+                    const int64_t *d_seg_ptr, int64_t nseg)
+{
+    Adj adj;
+    adj.row_ptr = d_row_ptr; adj.col = d_col; adj.val = d_val; adj.seg_row = d_seg_row; adj.seg_ptr = d_seg_ptr; adj.nseg = nseg;
+    adj.n = 0;
+    return adj;
+}
+
+// mirror[e] = the slot of (c, r) for the slot e = (r, c) of a CSR with ascending columns per row; -1 when it is missing
+__global__ void ngcf_mirror_kernel(const int64_t *__restrict__ row_ptr, const int32_t *__restrict__ col, long long n,
+                                   long long nnz, int32_t *__restrict__ mirror)
+{
+    for (long long e = (long long)blockIdx.x * blockDim.x + threadIdx.x; e < nnz; e += (long long)gridDim.x * blockDim.x) {
+        long long lo = 0, hi = n;                          // row of e: the last r with row_ptr[r] <= e
+        while (hi - lo > 1) {
+            const long long mid = (lo + hi) >> 1;
+            if (row_ptr[mid] <= e) lo = mid; else hi = mid;
+        }
+        const int r = (int)lo, c = col[e];
+        long long b = row_ptr[c], t = row_ptr[c + 1];      // r among the columns of row c
+        while (b < t) {
+            const long long mid = (b + t) >> 1;
+            if (col[mid] < r) b = mid + 1; else t = mid;
+        }
+        mirror[e] = (b < row_ptr[c + 1] && col[b] == r) ? (int32_t)b : -1;
+    }
+}
+
+// test hook: one forward's Philox masks, written by the functions the kernels call
+__global__ void ngcf_philox_masks_kernel(MsgDrop md, EdgeDrop ed, long long n, NgcfDims q, long long nnz,
+                                         uint8_t *__restrict__ keep, uint8_t *__restrict__ edge_keep)
+{
+    long long msg = 0;
+    for (int l = 0; l < q.L; ++l) msg += n * q.d[l + 1];
+    for (long long k = (long long)blockIdx.x * blockDim.x + threadIdx.x; k < msg + nnz; k += (long long)gridDim.x * blockDim.x) {
+        if (k >= msg) {
+            uint32_t words[4];
+            const unsigned long long e = (unsigned long long)(k - msg);
+            edge_words(ed, e >> 2, words);
+            edge_keep[e] = drop_kept(philox_word(words, (unsigned)(e & 3)), ed.thresh) ? 1 : 0;
+            continue;
+        }
+        long long base = 0;
+        int l = 0;
+        while (k - base >= n * q.d[l + 1]) { base += n * q.d[l + 1]; ++l; }
+        const long long r = (k - base) / q.d[l + 1];
+        const int o = (int)(k - base - r * q.d[l + 1]);
+        keep[k] = ngcf_drop_factor(nullptr, md, l, r, q.d[l + 1], o, 1.f) != 0.f ? 1 : 0;
+    }
 }
 
 }  // namespace drb
@@ -348,35 +456,78 @@ extern "C" int drb_ngcf_forward(const float *d_E0, const float *d_W, void *d_ws,
                                 const int32_t *d_seg_row, const int64_t *d_seg_ptr, int64_t nseg, int32_t tower_dtype,
                                 const uint8_t *d_keep, float dropout, float *d_out, void *stream)
 {
-    NgcfDims q;
     DRB_REQUIRE(d_keep == nullptr || (dropout > 0.f && dropout < 1.f), "ngcf: dropout masks need 0 < mess_dropout < 1");
-    DRB_REQUIRE(d_E0 && d_W && d_ws && d_row_ptr && d_out && ngcf_dims(q, U, I, dims, L), "ngcf_forward: bad arguments");
-    cudaStream_t st = (cudaStream_t)stream;
-    NgcfWs w;
-    carve_ngcf(d_ws, q, DRB_OPT_SGD, &w);
-    Adj adj;
-    adj.row_ptr = d_row_ptr; adj.col = d_col; adj.val = d_val; adj.seg_row = d_seg_row; adj.seg_ptr = d_seg_ptr; adj.nseg = nseg;
-    adj.n = q.n;
-    int rc = ngcf_forward(q, w, adj, d_E0, d_W, tower_dtype, st, d_keep, d_keep ? 1.0f / (float)(1.0 - (double)dropout) : 1.f);
-    if (rc != DRB_OK) return rc;
-    DRB_CUDA(cudaMemcpyAsync(d_out, w.ALL, sizeof(float) * (size_t)q.n * q.C, cudaMemcpyDeviceToDevice, st));
+    return ngcf_forward_call(d_E0, d_W, d_ws, U, I, dims, L, make_adj(d_row_ptr, d_col, d_val, d_seg_row, d_seg_ptr, nseg),
+                             tower_dtype, d_keep, d_keep ? 1.0f / (float)(1.0 - (double)dropout) : 1.f, make_msg_drop(0, 0, 0.f),
+                             nullptr, d_out, (cudaStream_t)stream);
+}
+
+// The same forward with the masks drawn on the device (dropout_engine 'philox'), keyed by (seed, forward).
+extern "C" int drb_ngcf_forward_philox(const float *d_E0, const float *d_W, void *d_ws, int32_t U, int32_t I, const int32_t *dims,
+                                       int32_t L, const int64_t *d_row_ptr, const int32_t *d_col, const float *d_val,
+                                       const int32_t *d_seg_row, const int64_t *d_seg_ptr, int64_t nseg, int32_t tower_dtype,
+                                       uint64_t seed, int64_t forward, float mess_dropout, double node_dropout, float *d_out,
+                                       void *stream)
+{
+    DRB_REQUIRE(mess_dropout >= 0.f && mess_dropout < 1.f, "ngcf: mess_dropout must be in [0, 1)");
+    DRB_REQUIRE(node_dropout >= 0.0 && node_dropout < 1.0, "ngcf: node_dropout must be in [0, 1)");
+    const EdgeDrop ed = make_edge_drop(seed, forward, node_dropout, nullptr);
+    return ngcf_forward_call(d_E0, d_W, d_ws, U, I, dims, L, make_adj(d_row_ptr, d_col, d_val, d_seg_row, d_seg_ptr, nseg),
+                             tower_dtype, nullptr, 1.0f / (float)(1.0 - (double)mess_dropout),
+                             make_msg_drop(seed, forward, mess_dropout), node_dropout > 0.0 ? &ed : nullptr, d_out,
+                             (cudaStream_t)stream);
+}
+
+extern "C" int drb_ngcf_edge_mirror(const int64_t *d_row_ptr, const int32_t *d_col, int64_t n, int64_t nnz, int32_t *d_mirror,
+                                    void *stream)
+{
+    DRB_REQUIRE(d_row_ptr && (nnz == 0 || (d_col && d_mirror)) && n > 0 && nnz >= 0 && nnz < (1ll << 31),
+                "ngcf_edge_mirror: bad arguments (at most 2^31 - 1 stored entries)");
+    if (nnz == 0) return DRB_OK;
+    ngcf_mirror_kernel<<<grid_for(nnz, 256), 256, 0, (cudaStream_t)stream>>>(d_row_ptr, d_col, n, nnz, d_mirror);
+    DRB_CUDA(cudaGetLastError());
     return DRB_OK;
 }
 
-// n_steps synchronous NGCF + BPR steps (apply != 0) or the loss of one batch (apply == 0), with the message dropout of :164
-// active when d_keep != NULL (reference default mess_dropout 0.1).  d_keep: per step the masks of the one forward() a step runs
-// (layers concatenated, bytes), steps concatenated; NULL = no dropout.
-extern "C" int drb_ngcf_bpr_train_steps(float *d_E0, float *d_W, void *d_ws, int32_t U, int32_t I, const int32_t *dims, int32_t L,
-                                        const int64_t *d_row_ptr, const int32_t *d_col, const float *d_val,
-                                        const int32_t *d_seg_row, const int64_t *d_seg_ptr, int64_t nseg, const int32_t *d_bu,
-                                        const int32_t *d_bi, const int32_t *d_bj, int64_t n_triples, int64_t batch,
-                                        int64_t first_step, int64_t n_steps, const drb_hyper *h, int64_t adam_step0,
-                                        int32_t apply, int32_t tower_dtype, const uint8_t *d_keep, float dropout,
-                                        double *d_step_loss, int32_t sync_and_check, int64_t *nan_step, void *stream)
+extern "C" int drb_ngcf_philox_masks(uint64_t seed, int64_t forward, int32_t U, int32_t I, const int32_t *dims, int32_t L,
+                                     float mess_dropout, double node_dropout, int64_t nnz, uint8_t *d_keep, uint8_t *d_edge_keep,
+                                     void *stream)
 {
     NgcfDims q;
-    DRB_REQUIRE(d_keep == nullptr || (dropout > 0.f && dropout < 1.f), "ngcf: dropout masks need 0 < mess_dropout < 1");
-    const float drop_scale = d_keep ? 1.0f / (float)(1.0 - (double)dropout) : 1.f;
+    DRB_REQUIRE(ngcf_dims(q, U, I, dims, L) && d_keep && (nnz == 0 || d_edge_keep) && nnz >= 0, "ngcf_philox_masks: bad arguments");
+    DRB_REQUIRE(mess_dropout >= 0.f && mess_dropout < 1.f && node_dropout >= 0.0 && node_dropout < 1.0,
+                "ngcf_philox_masks: dropout must be in [0, 1)");
+    long long total = nnz;
+    for (int l = 0; l < q.L; ++l) total += q.n * q.d[l + 1];
+    ngcf_philox_masks_kernel<<<grid_for(total, 256), 256, 0, (cudaStream_t)stream>>>(
+        make_msg_drop(seed, forward, mess_dropout), make_edge_drop(seed, forward, node_dropout, nullptr), q.n, q, nnz, d_keep,
+        d_edge_keep);
+    DRB_CUDA(cudaGetLastError());
+    return DRB_OK;
+}
+
+// The device masks of ngcf_train: message masks (mess > 0) and node dropout (node > 0; the backward needs the mirror index)
+// keyed by (seed, forward0 + step)
+struct NgcfPhilox {
+    bool on;
+    uint64_t seed;
+    int64_t forward0;
+    float mess;
+    double node;
+    const int32_t *mirror;
+};
+
+static int ngcf_train(float *d_E0, float *d_W, void *d_ws, int32_t U, int32_t I, const int32_t *dims, int32_t L,
+                      const int64_t *d_row_ptr, const int32_t *d_col, const float *d_val, const int32_t *d_seg_row,
+                      const int64_t *d_seg_ptr, int64_t nseg, const int32_t *d_bu, const int32_t *d_bi, const int32_t *d_bj,
+                      int64_t n_triples, int64_t batch, int64_t first_step, int64_t n_steps, const drb_hyper *h, int64_t adam_step0,
+                      int32_t apply, int32_t tower_dtype, const uint8_t *d_keep, float dropout, const NgcfPhilox &ph,
+                      double *d_step_loss, int32_t sync_and_check, int64_t *nan_step, void *stream)
+{
+    NgcfDims q;
+    const float drop_scale = d_keep ? 1.0f / (float)(1.0 - (double)dropout)
+                                    : ph.on ? 1.0f / (float)(1.0 - (double)ph.mess) : 1.f;
+    const bool node = ph.on && ph.node > 0.0;
     DRB_REQUIRE(d_E0 && d_W && d_ws && d_row_ptr && d_bu && d_bi && d_bj && h && d_step_loss, "ngcf_train_steps: null argument");
     DRB_REQUIRE(ngcf_dims(q, U, I, dims, L), "ngcf_train_steps: bad layer widths (1..256, 1 <= layers <= 8)");
     DRB_REQUIRE(batch > 0 && n_steps >= 0 && (n_steps == 0 || (first_step + n_steps - 1) * batch < n_triples),
@@ -398,7 +549,10 @@ extern "C" int drb_ngcf_bpr_train_steps(float *d_E0, float *d_W, void *d_ws, int
         size_t keep_per_step = 0;
         for (int l = 0; l < q.L; ++l) keep_per_step += (size_t)n * q.d[l + 1];
         const uint8_t *keep = d_keep ? d_keep + (size_t)s * keep_per_step : nullptr;
-        int rc = ngcf_forward(q, w, adj, d_E0, d_W, tower_dtype, st, keep, drop_scale);
+        const MsgDrop md = ph.on ? make_msg_drop(ph.seed, ph.forward0 + s, ph.mess) : make_msg_drop(0, 0, 0.f);
+        const EdgeDrop ed = make_edge_drop(ph.seed, ph.forward0 + s, ph.node, nullptr);
+        const EdgeDrop edT = make_edge_drop(ph.seed, ph.forward0 + s, ph.node, ph.mirror);   // A_drop^T for the backward
+        int rc = ngcf_forward(q, w, adj, d_E0, d_W, tower_dtype, st, keep, drop_scale, md, node ? &ed : nullptr);
         if (rc != DRB_OK) return rc;
         // phase 1: scores on the concatenated representation, norms on the ego rows, G = dL / d(representation)
         StepParams p = one_step(h, U, I, C, d_bu + base, d_bi + base, d_bj + base, nb, adam_step0 + s);
@@ -430,7 +584,7 @@ extern "C" int drb_ngcf_bpr_train_steps(float *d_E0, float *d_W, void *d_ws, int
             const uint8_t *keep_l = keep;
             if (keep_l) for (int k = 0; k < l; ++k) keep_l += (size_t)n * q.d[k + 1];
             ngcf_act_bwd_kernel<<<grid_for(n * 32, 256), 256, 0, st>>>(w.G, C, q.off[l + 1], dE, w.E[l + 1], w.Y[l], w.rn[l], n, out,
-                                                                     w.dY, keep_l, drop_scale);
+                                                                     w.dY, keep_l, drop_scale, md, l);
             DRB_CUDA(cudaGetLastError());
             rc = colsum_acc(w.dY, n, out, gb1, st);
             if (rc == DRB_OK) rc = colsum_acc(w.dY, n, out, gb2, st);
@@ -450,7 +604,8 @@ extern "C" int drb_ngcf_bpr_train_steps(float *d_E0, float *d_W, void *d_ws, int
             else
                 ngcf_mix_bwd_scalar_kernel<<<grid_for(n * in, 256), 256, 0, st>>>(w.dS, w.dT, El, w.X[l], n * in, dEl, w.dX);
             DRB_CUDA(cudaGetLastError());
-            rc = launch_spmm(adj, w.dX, w.AdX, nullptr, in, st);                                       // A_hat symmetric
+            rc = node ? launch_spmm_drop(adj, w.dX, w.AdX, in, edT, st)                               // A_drop^T dX
+                      : launch_spmm(adj, w.dX, w.AdX, nullptr, in, st);                                // A_hat symmetric
             if (rc != DRB_OK) return rc;
             if (l > 0) {
                 ngcf_add_kernel<<<grid_for(n * in, 256), 256, 0, st>>>(dEl, w.AdX, nullptr, 0, 0, n, in, dEl);
@@ -473,4 +628,41 @@ extern "C" int drb_ngcf_bpr_train_steps(float *d_E0, float *d_W, void *d_ws, int
     }
     if (sync_and_check) return check_nan(d_ws, st, nan_step);
     return DRB_OK;
+}
+
+// n_steps synchronous NGCF + BPR steps (apply != 0) or the loss of one batch (apply == 0), with the message dropout of :164
+// active when d_keep != NULL (reference default mess_dropout 0.1).  d_keep: per step the masks of the one forward() a step runs
+// (layers concatenated, bytes), steps concatenated; NULL = no dropout.
+extern "C" int drb_ngcf_bpr_train_steps(float *d_E0, float *d_W, void *d_ws, int32_t U, int32_t I, const int32_t *dims, int32_t L,
+                                        const int64_t *d_row_ptr, const int32_t *d_col, const float *d_val,
+                                        const int32_t *d_seg_row, const int64_t *d_seg_ptr, int64_t nseg, const int32_t *d_bu,
+                                        const int32_t *d_bi, const int32_t *d_bj, int64_t n_triples, int64_t batch,
+                                        int64_t first_step, int64_t n_steps, const drb_hyper *h, int64_t adam_step0,
+                                        int32_t apply, int32_t tower_dtype, const uint8_t *d_keep, float dropout,
+                                        double *d_step_loss, int32_t sync_and_check, int64_t *nan_step, void *stream)
+{
+    DRB_REQUIRE(d_keep == nullptr || (dropout > 0.f && dropout < 1.f), "ngcf: dropout masks need 0 < mess_dropout < 1");
+    const NgcfPhilox off = {false, 0, 0, 0.f, 0.0, nullptr};
+    return ngcf_train(d_E0, d_W, d_ws, U, I, dims, L, d_row_ptr, d_col, d_val, d_seg_row, d_seg_ptr, nseg, d_bu, d_bi, d_bj,
+                      n_triples, batch, first_step, n_steps, h, adam_step0, apply, tower_dtype, d_keep, dropout, off, d_step_loss,
+                      sync_and_check, nan_step, stream);
+}
+
+// The same steps with the masks drawn on the device (dropout_engine 'philox'): step s runs forward number forward0 + s.
+extern "C" int drb_ngcf_bpr_train_steps_philox(float *d_E0, float *d_W, void *d_ws, int32_t U, int32_t I, const int32_t *dims,
+                                               int32_t L, const int64_t *d_row_ptr, const int32_t *d_col, const float *d_val,
+                                               const int32_t *d_seg_row, const int64_t *d_seg_ptr, int64_t nseg,
+                                               const int32_t *d_bu, const int32_t *d_bi, const int32_t *d_bj, int64_t n_triples,
+                                               int64_t batch, int64_t first_step, int64_t n_steps, const drb_hyper *h,
+                                               int64_t adam_step0, int32_t apply, int32_t tower_dtype, uint64_t seed,
+                                               int64_t forward0, float mess_dropout, double node_dropout, const int32_t *d_mirror,
+                                               double *d_step_loss, int32_t sync_and_check, int64_t *nan_step, void *stream)
+{
+    DRB_REQUIRE(mess_dropout >= 0.f && mess_dropout < 1.f, "ngcf: mess_dropout must be in [0, 1)");
+    DRB_REQUIRE(node_dropout >= 0.0 && node_dropout < 1.0, "ngcf: node_dropout must be in [0, 1)");
+    DRB_REQUIRE(node_dropout == 0.0 || !apply || d_mirror, "ngcf: node dropout's backward needs the mirror index (drb_ngcf_edge_mirror)");
+    const NgcfPhilox ph = {true, seed, forward0, mess_dropout, node_dropout, d_mirror};
+    return ngcf_train(d_E0, d_W, d_ws, U, I, dims, L, d_row_ptr, d_col, d_val, d_seg_row, d_seg_ptr, nseg, d_bu, d_bi, d_bj,
+                      n_triples, batch, first_step, n_steps, h, adam_step0, apply, tower_dtype, nullptr, 0.f, ph, d_step_loss,
+                      sync_and_check, nan_step, stream);
 }

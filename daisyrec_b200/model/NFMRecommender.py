@@ -7,11 +7,15 @@ Factor tables ``embed_user.weight`` / ``embed_item.weight``, the first-order ter
 ``running`` (mean, var per BatchNorm).  Training goes through ``drb_nfm_bpr_train_steps``; rank / full_rank / predict score
 in eval mode (running statistics) through ``drb_nfm_scores`` + ``drb_topk_from_scores``.
 
-Dropout (``config['dropout']``, reference default 0.5, :67,:88): in train mode the host draws exactly the masks torch's Dropout
-modules would -- ``bernoulli_(1 - p)`` on the global CPU generator, forward(user, pos) first (FM_layers' Dropout, then the one
-behind each activation), then forward(user, neg) -- and uploads them as bytes with the batch, so a step equals the reference's
-and the global RNG ends where the reference's does.  That is a parity mechanism (one byte per activation and step through the
-host); ``dropout = 0`` is the throughput configuration.
+Dropout (``config['dropout']``, reference default 0.5, :67,:88) is active in train mode; eval-mode scoring is mask-free.  Where
+the masks come from (``dropout_engine``):
+- ``'auto'`` (default) / ``'torch'``: the host draws exactly the masks torch's Dropout modules would -- ``bernoulli_(1 - p)`` on
+  the global CPU generator, forward(user, pos) first (FM_layers' Dropout, then the one behind each activation), then
+  forward(user, neg) -- and uploads them as bytes with the batch, so a step equals the reference's and the global RNG ends where
+  the reference's does.  That is a parity mechanism (one byte per activation and step through the host).
+- ``'philox'``: the kernels draw the masks from Philox (same distribution, another stream), keyed by a seed -- one int64 drawn
+  from torch's global generator the first time a fit needs it -- and the global step; the pos and neg calls draw independent
+  masks and the backward regenerates them.  The throughput setting.
 
 Two reference behaviours are NOT mirrored because they are failures, not results: with ``dropout = 0`` today's torch makes
 the reference's own ``backward()`` raise (the in-place ``fm += ...`` of :120 aliases the activation output), and
@@ -39,6 +43,10 @@ class NFM(GeneralRecommender):
         self.dropout = float(config['dropout'] or 0.0)
         if not 0.0 <= self.dropout < 1.0:
             raise ValueError(f"dropout probability has to be in [0, 1), but got {self.dropout}")
+        self.dropout_engine = str(config.get('dropout_engine', 'auto')).lower()
+        if self.dropout_engine not in ('auto', 'torch', 'philox'):
+            raise ValueError(f"dropout_engine must be 'auto', 'torch' or 'philox', got {self.dropout_engine!r}")
+        self._philox_seed = None
         if self.act_function not in ops.NFM_ACT:
             raise NotImplementedError(f"act_function={self.act_function!r}: expected one of {sorted(ops.NFM_ACT)}")
         U, I, F, Ln = self.user_num, self.item_num, self.factors, self.num_layers
@@ -89,6 +97,15 @@ class NFM(GeneralRecommender):
         return ops.NfmWorkspace(self.user_num, self.item_num, self.factors, self.num_layers, self.batch_norm, opt, max(rows, 2),
                                 self.device)
 
+    def _begin_fit(self, opt):
+        self._philox_seed = None                                         # drawn lazily: a fit without device masks draws nothing
+        super()._begin_fit(opt)
+
+    def _drop_seed(self):
+        if self._philox_seed is None:
+            self._philox_seed = int(torch.empty((), dtype=torch.int64).random_().item())
+        return self._philox_seed
+
     def _host_keep(self, rows_per_step):
         """The masks nn.Dropout would draw for steps of rows_per_step[k] triples, drawn by torch on the global CPU generator in
         the reference's order -> uint8 CUDA tensor [step][forward call][site][rows][F] (drb_nfm_bpr_train_steps)."""
@@ -106,6 +123,9 @@ class NFM(GeneralRecommender):
         args = (self.embed_user.weight, self.embed_item.weight, self.bias, self.net, self.running, self._ws, self._act)
         if not (self.training and self.dropout > 0.0):
             return ops.nfm_bpr_train_steps(*args, bu, bi, bj, batch, first, n_steps, self._hp, **kw)
+        if self.dropout_engine == 'philox':
+            return ops.nfm_bpr_train_steps_philox(*args, bu, bi, bj, batch, first, n_steps, self._hp, dropout=self.dropout,
+                                                  seed=self._drop_seed(), **kw)
         per_step = 2 * (1 + self.num_layers) * batch * self.factors
         chunk = max(1, (64 << 20) // per_step)                           # at most 64 MB of masks per call
         out, s = [], first

@@ -1,5 +1,5 @@
 """NGCF + BPR on the GPU path, with the reference's class name, config keys and methods
-(daisy/model/NGCFRecommender.py:61-252; node_dropout = 0).
+(daisy/model/NGCFRecommender.py:61-252).
 
 The ego table E0 = cat(embed_user.weight, embed_item.weight) is one contiguous device tensor; the BiGNN layers live in
 one flat fp32 block (``gnn``: per layer W1, b1, W2, b2 in module-registration order); the normalised adjacency is
@@ -10,10 +10,20 @@ optimiser phases); rank / full_rank / predict score the cached concatenated repr
 
 Message dropout (``mess_dropout``, reference default 0.1): forward() builds ``nn.Dropout(mess_dropout)`` per layer (:164), a
 module in training mode, so the reference drops on EVERY forward() -- the one behind rank() / full_rank() / predict() as well.
-The host draws exactly those masks (one ``bernoulli_(1 - p)`` per layer over its [n, width] output, torch's global CPU
-generator) and uploads them as bytes; the kernels apply them between LeakyReLU and the row normalisation, forward and backward.
-That is a parity mechanism (one byte per node and width through the host per forward); ``mess_dropout = 0`` is the throughput
-configuration.  ``node_dropout`` (reference default 0; a sparse dropout of the adjacency) is refused when non-zero.
+Node dropout (``node_dropout``, reference default 0): ``SparseDropout`` (:19-35) keeps every stored entry of the adjacency with
+probability 1 - p and scales it by 1 / (1 - p), once per forward() and only in train mode (fit's steps, train_step, calc_loss
+and forward() while ``model.training``; fit ends each epoch in eval mode, so rank() after fit drops messages but not edges).
+
+Where the masks come from (``dropout_engine``):
+- ``'auto'`` (default) / ``'torch'``: the host draws exactly the reference's message masks (one ``bernoulli_(1 - p)`` per layer
+  over its [n, width] output, torch's global CPU generator) and uploads them as bytes; the kernels apply them between LeakyReLU
+  and the row normalisation, forward and backward.  That is a parity mechanism (one byte per node and width through the host
+  per forward).  ``node_dropout`` must be 0 here: host parity would need 2 * nnz host draws per forward.
+- ``'philox'``: message and node masks are drawn inside the kernels from Philox (same distributions, another stream), keyed by
+  a seed -- one int64 drawn from torch's global generator the first time a fit needs it -- and the model's forward counter,
+  which advances once per forward(): once per training step and once per scoring forward, so the masks do not depend on
+  ``steps_per_launch``.  The backward regenerates the message masks and multiplies by the transpose of the dropped adjacency
+  through the CSR's mirror index (``LgcnGraph.edge_mirror``, built once when node dropout is on).
 """
 import numpy as np
 import torch
@@ -35,9 +45,17 @@ class NGCF(GeneralRecommender):
         self.hidden_size_list = [self.embedding_size] + list(hidden)
         self.node_dropout = config['node_dropout']
         self.message_dropout = config['mess_dropout']
-        if float(self.node_dropout or 0.0) != 0.0:
-            raise NotImplementedError('NGCF on the GPU path runs with node_dropout = 0 (the reference default; a sparse dropout '
-                                      'of the adjacency drawn from the torch RNG)')
+        engine = str(config.get('dropout_engine', 'auto')).lower()
+        if engine not in ('auto', 'torch', 'philox'):
+            raise ValueError(f"dropout_engine must be 'auto', 'torch' or 'philox', got {engine!r}")
+        self.dropout_engine = engine
+        if engine == 'philox':
+            self.node_dropout = float(self.node_dropout or 0.0)
+            if not 0.0 <= self.node_dropout < 1.0:
+                raise ValueError(f"node_dropout has to be in [0, 1), but got {self.node_dropout}")
+        elif float(self.node_dropout or 0.0) != 0.0:
+            raise NotImplementedError('NGCF on the GPU path runs node_dropout only with dropout_engine=\'philox\' (the reference '
+                                      'draws its sparse dropout of the adjacency from the torch RNG)')
         self.message_dropout = float(self.message_dropout or 0.0)
         if not 0.0 <= self.message_dropout < 1.0:
             raise ValueError(f"dropout probability has to be in [0, 1), but got {self.message_dropout}")
@@ -76,6 +94,8 @@ class NGCF(GeneralRecommender):
         if td not in ('fp32', 'bf16'):
             raise ValueError(f"tower_dtype must be 'fp32' or 'bf16', got {td!r}")
         self._tower_dtype = 1 if td == 'bf16' else 0
+        self._forwards = 0                                           # forward() calls so far: the Philox masks' counter
+        self._philox_seed = None
 
     def _workspace(self, opt, rows=None):
         return ops.NgcfWorkspace(self.user_num, self.item_num, self.hidden_size_list, opt, self.device)
@@ -92,8 +112,33 @@ class NGCF(GeneralRecommender):
                 parts.append(torch.empty(n, int(width), dtype=torch.float32).bernoulli_(keep).to(torch.uint8).reshape(-1))
         return torch.cat(parts).to(self.device)
 
+    def _begin_fit(self, opt):
+        self._philox_seed = None                                     # drawn lazily: a fit without device masks draws nothing
+        super()._begin_fit(opt)
+
+    def _philox(self):
+        """-> (seed, node dropout of this forward) when the masks come from the device, else None."""
+        node = self.node_dropout if self.training else 0.0           # SparseDropout is the identity in eval mode (:30-31)
+        if self.dropout_engine != 'philox' or (self.message_dropout <= 0.0 and node <= 0.0):
+            return None
+        if self._philox_seed is None:
+            self._philox_seed = int(torch.empty((), dtype=torch.int64).random_().item())
+        return self._philox_seed, node
+
+    def _next_forwards(self, k):
+        first = self._forwards
+        self._forwards += k
+        return first
+
     def _launch(self, bu, bi, bj, batch, first, n_steps, apply=True):
         self._drop_cache()                                           # NGCFRecommender.py:175-176
+        ph = self._philox()
+        if ph is not None:
+            return ops.ngcf_bpr_train_steps_philox(self.E0, self.gnn, self._ws, self.graph, bu, bi, bj, batch, first, n_steps,
+                                                   self._hp, adam_step0=self._opt_steps if apply else 0, apply=apply,
+                                                   tower_dtype=self._tower_dtype, seed=ph[0],
+                                                   forward0=self._next_forwards(1 if not apply else n_steps),
+                                                   mess_dropout=self.message_dropout, node_dropout=ph[1])
         kw = dict(apply=apply, tower_dtype=self._tower_dtype, dropout=self.message_dropout)
         if self.message_dropout <= 0.0:
             return ops.ngcf_bpr_train_steps(self.E0, self.gnn, self._ws, self.graph, bu, bi, bj, batch, first, n_steps, self._hp,
@@ -111,6 +156,11 @@ class NGCF(GeneralRecommender):
     def forward(self):
         """NGCFRecommender.py:157-172 -> (user_all_embeddings, item_all_embeddings): the concatenated layer outputs."""
         self._ensure()
+        ph = self._philox()
+        if ph is not None:
+            rep = ops.ngcf_forward_philox(self.E0, self.gnn, self._ws, self.graph, self._tower_dtype, seed=ph[0],
+                                          forward=self._next_forwards(1), mess_dropout=self.message_dropout, node_dropout=ph[1])
+            return rep[:self.user_num], rep[self.user_num:]
         rep = ops.ngcf_forward(self.E0, self.gnn, self._ws, self.graph, self._tower_dtype, dropout=self.message_dropout,
                                keep=self._host_keep(1))              # the reference's forward() always drops (:164)
         return rep[:self.user_num], rep[self.user_num:]

@@ -574,9 +574,22 @@ class LgcnGraph:
             self.val = torch.from_numpy(np.ascontiguousarray(val, np.float32)).to(device)
         self.seg_row = torch.from_numpy(seg_row).to(device)
         self.seg_ptr = torch.from_numpy(seg_ptr).to(device)
+        self.mirror = None
 
     def args(self):
         return (_ptr(self.row_ptr), _ptr(self.col), _ptr(self.val), _ptr(self.seg_row), _ptr(self.seg_ptr), self.nseg)
+
+    def edge_mirror(self):
+        """int32 [nnz]: the CSR slot of (c, r) for every slot (r, c), built once on the device (NGCF's node-dropout backward
+        multiplies by the transpose of the dropped adjacency through it).  ValueError when A is not structurally symmetric."""
+        if self.mirror is None:
+            nnz = int(self.row_ptr[-1].item())
+            m = torch.empty(max(nnz, 1), dtype=torch.int32, device=self.row_ptr.device)
+            L.check(L.lib().drb_ngcf_edge_mirror(_ptr(self.row_ptr), _ptr(self.col), self.n, nnz, _ptr(m), _stream()))
+            if nnz and bool((m[:nnz] < 0).any()):
+                raise ValueError("node dropout needs a structurally symmetric adjacency")
+            self.mirror = m
+        return self.mirror
 
 
 class LgcnWorkspace:
@@ -661,6 +674,41 @@ def ngcf_bpr_train_steps(E0, W, ws, graph, bu, bi, bj, batch, first_step, n_step
                         None if keep is None else _ptr(keep), C.c_float(dropout if keep is not None else 0.0))
 
 
+def ngcf_forward_philox(E0, W, ws, graph, tower_dtype=0, seed=0, forward=0, mess_dropout=0.0, node_dropout=0.0):
+    """forward number ``forward`` with the Philox masks of ``seed``: message dropout, and node dropout when node_dropout > 0."""
+    _dev(E0, torch.float32, "E0"); _dev(W, torch.float32, "W")
+    out = torch.empty((ws.U + ws.I, sum(ws.dims)), dtype=torch.float32, device=E0.device)
+    L.check(L.lib().drb_ngcf_forward_philox(_ptr(E0), _ptr(W), _ptr(ws.buf), ws.U, ws.I, _dims_arr(ws.dims), len(ws.dims) - 1,
+                                            *graph.args(), tower_dtype, C.c_uint64(seed), int(forward), C.c_float(mess_dropout),
+                                            C.c_double(node_dropout), _ptr(out), _stream()))
+    return out
+
+
+def ngcf_bpr_train_steps_philox(E0, W, ws, graph, bu, bi, bj, batch, first_step, n_steps, hp, adam_step0=0, apply=True,
+                                check=True, tower_dtype=0, seed=0, forward0=0, mess_dropout=0.0, node_dropout=0.0):
+    """NGCF steps with the Philox masks of ``seed``; step s runs forward number forward0 + s."""
+    _dev(E0, torch.float32, "E0"); _dev(W, torch.float32, "W")
+    for t, nm in ((bu, "bu"), (bi, "bi"), (bj, "bj")):
+        _dev(t, torch.int32, nm)
+    mirror = graph.edge_mirror() if node_dropout > 0.0 and apply else None
+    return _train_steps(L.lib().drb_ngcf_bpr_train_steps_philox, n_steps, E0.device, check, _ptr(E0), _ptr(W), _ptr(ws.buf), ws.U,
+                        ws.I, _dims_arr(ws.dims), len(ws.dims) - 1, *graph.args(), _ptr(bu), _ptr(bi), _ptr(bj), bu.numel(), batch,
+                        first_step, n_steps, C.byref(hp), adam_step0, 1 if apply else 0, tower_dtype, C.c_uint64(seed),
+                        int(forward0), C.c_float(mess_dropout), C.c_double(node_dropout),
+                        None if mirror is None else _ptr(mirror))
+
+
+def ngcf_philox_masks(seed, forward, user_num, item_num, dims, mess_dropout, node_dropout, nnz, device):
+    """test hook: forward number ``forward``'s message masks (uint8, layers concatenated as ``keep``) and edge keep (uint8 [nnz])"""
+    dims = [int(d) for d in dims]
+    keep = torch.empty((user_num + item_num) * sum(dims[1:]), dtype=torch.uint8, device=device)
+    edge = torch.empty(max(int(nnz), 1), dtype=torch.uint8, device=device)
+    L.check(L.lib().drb_ngcf_philox_masks(C.c_uint64(seed), int(forward), user_num, item_num, _dims_arr(dims), len(dims) - 1,
+                                          C.c_float(mess_dropout), C.c_double(node_dropout), int(nnz), _ptr(keep), _ptr(edge),
+                                          _stream()))
+    return keep, edge[:int(nnz)]
+
+
 # ------------------------------------------------------------------ NFM
 NFM_ACT = {"relu": 0, "sigmoid": 1, "tanh": 2}
 
@@ -699,6 +747,29 @@ def nfm_bpr_train_steps(P, Q, bias, N, Rs, ws, act, bu, bi, bj, batch, first_ste
         None if Rs is None or Rs.numel() == 0 else _ptr(Rs), _ptr(ws.buf), ws.U, ws.I, ws.F, ws.Ln, ws.bn, act, ws.max_rows, _ptr(bu),
         _ptr(bi), _ptr(bj), bu.numel(), batch, first_step, n_steps, C.byref(hp), adam_step0, 1 if apply else 0, tower_dtype,
         None if keep is None else _ptr(keep), C.c_float(dropout if keep is not None else 0.0))
+
+
+def nfm_bpr_train_steps_philox(P, Q, bias, N, Rs, ws, act, bu, bi, bj, batch, first_step, n_steps, hp, adam_step0=0, apply=True,
+                               check=True, tower_dtype=0, dropout=0.0, seed=0):
+    """NFM steps with the Dropout masks drawn on the device from Philox: step s keyed by (seed, adam_step0 + s)."""
+    for t in (P, Q, bias, N):
+        _dev(t, torch.float32, "parameter")
+    for t, nm in ((bu, "bu"), (bi, "bi"), (bj, "bj")):
+        _dev(t, torch.int32, nm)
+    return _train_steps(
+        L.lib().drb_nfm_bpr_train_steps_philox, n_steps, P.device, check, _ptr(P), _ptr(Q), _ptr(bias), _ptr(N),
+        None if Rs is None or Rs.numel() == 0 else _ptr(Rs), _ptr(ws.buf), ws.U, ws.I, ws.F, ws.Ln, ws.bn, act, ws.max_rows, _ptr(bu),
+        _ptr(bi), _ptr(bj), bu.numel(), batch, first_step, n_steps, C.byref(hp), adam_step0, 1 if apply else 0, tower_dtype,
+        C.c_float(dropout), C.c_uint64(seed))
+
+
+def nfm_philox_masks(seed, step, rows, factors, num_layers, dropout, device):
+    """test hook: step ``step``'s Philox masks for a batch of ``rows`` triples, uint8 [2 * (1 + num_layers) * rows * factors] in
+    the layout of ``keep``"""
+    out = torch.empty(2 * (1 + num_layers) * rows * factors, dtype=torch.uint8, device=device)
+    L.check(L.lib().drb_nfm_philox_masks(C.c_uint64(seed), int(step), int(rows), factors, num_layers, C.c_float(dropout), _ptr(out),
+                                         _stream()))
+    return out
 
 
 def nfm_scores(P, Q, bias, N, Rs, ws, act, u, i, tower_dtype=0):

@@ -280,7 +280,7 @@ int drb_fm_full_rank(const float *d_P, const float *d_Q, const float *d_bias, in
 int drb_fm_predict(const float *d_P, const float *d_Q, const float *d_bias, int32_t user_num, int32_t item_num,
                    int32_t factors, const int32_t *d_u, const int32_t *d_i, int64_t n, float *d_out, void *stream);
 
-/* ---- NGCF + BPR (daisy/model/NGCFRecommender.py:38-252; SURVEY 8(f) rank 4; node_dropout = 0) -------------------------
+/* ---- NGCF + BPR (daisy/model/NGCFRecommender.py:38-252; SURVEY 8(f) rank 4) ---------------------------------------------
  * E0: the ego table cat(embed_user, embed_item) [(U+I), dims[0]];  dims[0..L]: embedding size then hidden_size_list;
  * W: flat fp32 block, per BiGNN layer W1 [out,in], b1 [out], W2 [out,in], b2 [out] (linear, interact_transform; :46-47);
  * adjacency: the normalised CSR + segment list of drb_lgcn_* (get_norm_adj_mat :125-146 is LightGCN's).
@@ -306,6 +306,37 @@ int drb_ngcf_bpr_train_steps(float *d_E0, float *d_W, void *d_ws, int32_t user_n
                              int64_t n_steps, const drb_hyper *hyper, int64_t adam_step0, int32_t apply, int32_t tower_dtype,
                              const uint8_t *d_keep, float mess_dropout, double *d_step_loss, int32_t sync_and_check,
                              int64_t *nan_step, void *stream);
+/* dropout_engine 'philox': the masks are drawn inside the kernels from Philox4x32-10 keyed by (seed, forward counter) with the
+ * keep rule NeuMF uses (kept iff the Philox word >= p * 2^32, kept values scaled by 1 / (1 - p)):
+ *   message masks   element (r, o) of layer l's output: word o % 4 of the counter (o / 4, r, l, forward); the backward
+ *                   regenerates them;
+ *   node dropout    (node_dropout > 0, the reference's SparseDropout) CSR slot e of A_hat: word e % 4 of (e / 4, 0x80000000,
+ *                   forward); a kept entry weighs val * (float)(1 / (1 - node_dropout)), a dropped one nothing.  One edge mask
+ *                   per forward serves every layer.  The backward multiplies by A_drop^T through d_mirror (drb_ngcf_edge_mirror).
+ * drb_ngcf_forward_philox          forward number `forward` (rank / full_rank / predict; node_dropout > 0 only in train mode).
+ * drb_ngcf_bpr_train_steps_philox  step s runs forward number forward0 + s, so the masks do not depend on how steps are grouped
+ *                                  into calls.  d_mirror is needed when node_dropout > 0 and apply != 0.
+ * drb_ngcf_edge_mirror     mirror[e] = the slot of (c, r) for the slot e = (r, c) of a CSR with ascending columns per row, -1 when
+ *                          (c, r) is not stored.
+ * drb_ngcf_philox_masks    test hook: one forward's message masks as bytes in d_keep's layout (layers concatenated) and the edge
+ *                          keep of every CSR slot (1 = kept) in d_edge_keep [nnz]. */
+int drb_ngcf_forward_philox(const float *d_E0, const float *d_W, void *d_ws, int32_t user_num, int32_t item_num,
+                            const int32_t *h_dims, int32_t num_layers, const int64_t *d_row_ptr, const int32_t *d_col,
+                            const float *d_val, const int32_t *d_seg_row, const int64_t *d_seg_ptr, int64_t nseg,
+                            int32_t tower_dtype, uint64_t seed, int64_t forward, float mess_dropout, double node_dropout,
+                            float *d_out, void *stream);
+int drb_ngcf_bpr_train_steps_philox(float *d_E0, float *d_W, void *d_ws, int32_t user_num, int32_t item_num, const int32_t *h_dims,
+                                    int32_t num_layers, const int64_t *d_row_ptr, const int32_t *d_col, const float *d_val,
+                                    const int32_t *d_seg_row, const int64_t *d_seg_ptr, int64_t nseg, const int32_t *d_bu,
+                                    const int32_t *d_bi, const int32_t *d_bj, int64_t n, int64_t batch, int64_t first_step,
+                                    int64_t n_steps, const drb_hyper *hyper, int64_t adam_step0, int32_t apply, int32_t tower_dtype,
+                                    uint64_t seed, int64_t forward0, float mess_dropout, double node_dropout,
+                                    const int32_t *d_mirror, double *d_step_loss, int32_t sync_and_check, int64_t *nan_step,
+                                    void *stream);
+int drb_ngcf_edge_mirror(const int64_t *d_row_ptr, const int32_t *d_col, int64_t n, int64_t nnz, int32_t *d_mirror, void *stream);
+int drb_ngcf_philox_masks(uint64_t seed, int64_t forward, int32_t user_num, int32_t item_num, const int32_t *h_dims,
+                          int32_t num_layers, float mess_dropout, double node_dropout, int64_t nnz, uint8_t *d_keep,
+                          uint8_t *d_edge_keep, void *stream);
 
 /* ---- NFM + BPR (daisy/model/NFMRecommender.py:14-209; SURVEY 8(f) rank 4) ------------------------------------------
  * P [U,F], Q [I,F] factor tables; d_bias = packed [u_bias (U), i_bias (I), bias_];
@@ -332,6 +363,18 @@ int drb_nfm_bpr_train_steps(float *d_P, float *d_Q, float *d_bias, float *d_N, f
                             int64_t batch, int64_t first_step, int64_t n_steps, const drb_hyper *hyper, int64_t adam_step0,
                             int32_t apply, int32_t tower_dtype, const uint8_t *d_keep, float dropout, double *d_step_loss,
                             int32_t sync_and_check, int64_t *nan_step, void *stream);
+/* drb_nfm_bpr_train_steps_philox  the same steps with dropout_engine 'philox': the masks are drawn inside the kernels, element
+ *    (t, f) of forward call c (0 pos, 1 neg) at site k is kept iff word f % 4 of Philox4x32-10(seed; f / 4, t, k | c << 8,
+ *    adam_step0 + s) >= dropout * 2^32 (NeuMF's keep rule); the backward regenerates them.  dropout = 0: no dropout.
+ * drb_nfm_philox_masks  test hook: the masks of step `step` for a batch of `rows` triples as bytes in d_keep's layout. */
+int drb_nfm_bpr_train_steps_philox(float *d_P, float *d_Q, float *d_bias, float *d_N, float *d_Rs, void *d_ws, int32_t user_num,
+                                   int32_t item_num, int32_t factors, int32_t num_layers, int32_t batch_norm, int32_t act,
+                                   int64_t max_rows, const int32_t *d_bu, const int32_t *d_bi, const int32_t *d_bj, int64_t n,
+                                   int64_t batch, int64_t first_step, int64_t n_steps, const drb_hyper *hyper, int64_t adam_step0,
+                                   int32_t apply, int32_t tower_dtype, float dropout, uint64_t seed, double *d_step_loss,
+                                   int32_t sync_and_check, int64_t *nan_step, void *stream);
+int drb_nfm_philox_masks(uint64_t seed, int64_t step, int64_t rows, int32_t factors, int32_t num_layers, float dropout,
+                         uint8_t *d_keep, void *stream);
 int drb_nfm_scores(const float *d_P, const float *d_Q, const float *d_bias, const float *d_N, const float *d_Rs, void *d_ws,
                    int32_t user_num, int32_t item_num, int32_t factors, int32_t num_layers, int32_t batch_norm, int32_t act,
                    int32_t opt, int64_t max_rows, const int32_t *d_u, const int32_t *d_i, int64_t n, int32_t tower_dtype,
