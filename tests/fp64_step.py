@@ -319,9 +319,10 @@ def checked_step(st, lo, nb, batch, tag, adam_step0=0, apply=True, ref_device="c
     return (rec, res) if with_res else rec
 
 
-def launch_vs_singles(multi, single, n, batch, k, first_step=0, states=True, ref_device="cuda", **step):
+def launch_vs_singles(multi, single, n, batch, k, first_step=0, states=True, ref_device="cuda", step_of=None, **step):
     """one k-step launch of `multi` (rows [0, n), steps first_step ..) against k single launches of `single` from the same
-    start, each checked against the reference -> the singles' records and one record of the launch: each launch step's loss
+    start, each checked against the reference (with the per-step inputs `step`, or step_of(s) for step s when given: each
+    step's own dropout masks) -> the singles' records and one record of the launch: each launch step's loss
     within the bound of the single's reference, and (states) the launch's end state within the singles' end state plus twice
     the sum of their per-step half-widths 2 u |theta| + lr (KAPPA u N + P) (both runs lie within the bound of the same
     exact trajectory), every element of every parameter tensor"""
@@ -330,7 +331,7 @@ def launch_vs_singles(multi, single, n, batch, k, first_step=0, states=True, ref
     for s in range(first_step, first_step + k):
         pre = single.snapshot()
         r, res = checked_step(single, s * batch, min(batch, n - s * batch), batch, f"single {s}", adam_step0=s,
-                              ref_device=ref_device, with_res=True, **step)
+                              ref_device=ref_device, with_res=True, **(step if step_of is None else step_of(s)))
         recs.append(r)
         lrat.append(abs(float(losses[s - first_step]) - res["loss"]) / (single.kappa * U_RND * res["lossN"] + res["lossP"]))
         for key in res["g"]:

@@ -7,6 +7,9 @@ regulariser on the EGO rows counted per occurrence, backward = the same propagat
 X = A E, [S | T] = [E + X | X * E], y = S W1^T + b1 + T W2^T + b2, z = LeakyReLU_0.2(y), E' = z / max(||z||, 1e-12); scores on
 cat(E_0 .. E_L), the same regulariser on the ego rows, the normalise / LeakyReLU backward of ngcf_act_bwd_kernel.  With
 tower_dtype 1 every BiGNN GEMM (N <= 256 always holds) rounds its two operands to bf16 (emulated from the fp32 bits).
+`ngcf_ref` also takes one forward's dropout masks (message keep bytes, node keep bytes over the CSR slots with
+RefGraph.dropped_by); without them it is the reference above, unchanged.  test_gpu_ngcf_dropout_fp64.py runs the dropout
+cases.
 
 N_e runs the chain on |E|, |W|, |G| (A is non-negative).  P_e: LightGCN has none (its bound is pure KAPPA); NGCF has
 LeakyReLU gates whose pre-activation lies within its noise of 0 (slope 1 against 0.2 in the backward) and, in bf16, operands
@@ -114,6 +117,25 @@ class RefGraph:
         self.row_ptr, self.col, self.val = rp, cl, vl
         self.device = device
         self.A = {dt: torch.sparse_csr_tensor(rp, cl, vl.to(dt), size=(self.n, self.n)).to(device) for dt in (F64, torch.float32)}
+        self.T = self                   # A_hat is symmetric: the backward multiplies by A_hat itself
+        self._tperm = None
+
+    def dropped_by(self, edge, p):
+        """node dropout (the reference's SparseDropout) with the keep bytes `edge` over the CSR slots: a graph whose kept slots
+        weigh val * (float)(1 / (1 - p)) in fp32 and whose dropped slots weigh 0, with its transpose as .T (A_drop is not
+        symmetric); both as float64 and float32 CSR"""
+        kept = torch.as_tensor(edge).to("cpu", torch.bool)
+        assert kept.numel() == self.col.numel()
+        vl = torch.where(kept, self.val * torch.tensor(np.float32(1.0 / (1.0 - p))), torch.zeros((), dtype=torch.float32))
+        if self._tperm is None:          # the slots in (col, row) order: the transpose's CSR order
+            rows = torch.repeat_interleave(torch.arange(self.n), self.row_ptr[1:] - self.row_ptr[:-1])
+            self._tperm = torch.argsort(self.col * self.n + rows)
+            self._trows = rows[self._tperm]
+            self._tptr = torch.cat([torch.zeros(1, dtype=torch.int64), torch.cumsum(torch.bincount(self.col, minlength=self.n), 0)])
+        g = RefGraph(self.row_ptr, self.col, vl, self.device)
+        g.T = RefGraph(self._tptr, self._trows, vl[self._tperm], self.device)
+        g.T.T = g
+        return g
 
     def dropped(self):
         """the same graph with the last edge of the first multi-segment row removed (a defect of the backward only)"""
@@ -126,6 +148,7 @@ class RefGraph:
         g.n, g.row_ptr, g.col, g.val, g.device = self.n, self.row_ptr, self.col, vl, self.device
         g.A = {dt: torch.sparse_csr_tensor(self.row_ptr, self.col, vl.to(dt), size=(self.n, self.n)).to(self.device)
                for dt in (F64, torch.float32)}
+        g.T = g
         g.dropped_row = r
         return g
 
@@ -228,8 +251,27 @@ def ngcf_layout(dims):
     return out, o
 
 
-def ngcf_ref(E0, W, U, g, dims, bu, bi, bj, reg=(0.0, 0.0), tower_dtype=0, dt=F64, defects=(), kappa=None):
-    """one NGCF + BPR step (gradients of E0 and W, not applied) -> dict(gE, NE, PE, gW, NW, PW, loss, lossN, lossP, ALL...)"""
+def msg_scale(p):
+    """the kernels' message-dropout factor 1.0f / (float)(1 - (double)p) of an fp32 p"""
+    return float(np.float32(1.0) / np.float32(1.0 - float(np.float32(p))))
+
+
+def msg_factors(keep, dims, n, p, dt, device):
+    """one forward's message keep bytes (layers concatenated, [n, d_l] each) -> per-layer factors keep * msg_scale(p)"""
+    k = torch.as_tensor(keep).to(device)
+    out, o = [], 0
+    for w in dims[1:]:
+        out.append(k[o:o + n * w].view(n, w).to(dt) * msg_scale(p))
+        o += n * w
+    assert o == k.numel()
+    return out
+
+
+def ngcf_ref(E0, W, U, g, dims, bu, bi, bj, reg=(0.0, 0.0), tower_dtype=0, dt=F64, defects=(), kappa=None, keep=None, p=0.0,
+             edge=None, node_p=0.0):
+    """one NGCF + BPR step (gradients of E0 and W, not applied) -> dict(gE, NE, PE, gW, NW, PW, loss, lossN, lossP, ALL...).
+    keep (message dropout p): the keep bytes of one forward, layers concatenated; edge (node dropout node_p): the keep bytes
+    of the CSR slots of g, one mask for every layer.  The masks are given, so they add no P_e term."""
     st = Flags(kappa_of("ngcf", tower_dtype) if kappa is None else kappa)
     ku = st.k * U_RND
     dev = E0.device
@@ -237,8 +279,14 @@ def ngcf_ref(E0, W, U, g, dims, bu, bi, bj, reg=(0.0, 0.0), tower_dtype=0, dt=F6
     lay, nW = ngcf_layout(dims)
     Wd = W.to(dt)
     bf = tower_dtype == 1
-    keep = lambda op, l: bf and not (f"unrounded_{op}" in defects and l == 0)     # a defect: one operand of layer 0 stays fp32
+    keep_bf = lambda op, l: bf and not (f"unrounded_{op}" in defects and l == 0)  # a defect: one operand of layer 0 stays fp32
     Z = lambda t: torch.zeros(t.shape, dtype=F64, device=dev)
+    mf = None if keep is None else msg_factors(keep, dims, E0.shape[0], p, dt, dev)
+    gl = [g] * L                                     # the adjacency of each layer: A_hat, or A_drop (.T: its transpose)
+    if edge is not None:
+        gl = [g.dropped_by(edge, 0.0 if "node_unscaled" in defects else node_p)] * L   # a defect: kept slots keep val
+        if "node_mask_per_layer" in defects:         # a defect: every layer but the first draws its own edge mask
+            gl = [gl[0]] + [g.dropped_by(np.random.default_rng(l).random(g.col.numel()) >= node_p, node_p) for l in range(1, L)]
     E, EN, EP = E0.to(dt), Z(E0), Z(E0)
     acts = []
     for l in range(L):
@@ -246,14 +294,14 @@ def ngcf_ref(E0, W, U, g, dims, bu, bi, bj, reg=(0.0, 0.0), tower_dtype=0, dt=F6
         W1 = Wd[lay[l]["W1"][0]:lay[l]["W1"][1]].view(p, i)
         W2 = Wd[lay[l]["W2"][0]:lay[l]["W2"][1]].view(p, i)
         b1, b2 = Wd[lay[l]["b1"][0]:lay[l]["b1"][1]], Wd[lay[l]["b2"][0]:lay[l]["b2"][1]]
-        X = spmm(g, E, dt)
-        XN, XP = spmm(g, _A(E) + EN, F64), spmm(g, EP, F64)
+        X = spmm(gl[l], E, dt)
+        XN, XP = spmm(gl[l], _A(E) + EN, F64), spmm(gl[l], EP, F64)
         S, SN, SP = E + X, EN + XN + _A(E + X), EP + XP
         T, TN, TP = X * E, _A(X) * EN + XN * _A(E) + _A(X * E), _A(X) * EP + XP * _A(E)
-        Sr, SrN, SrP = rnd(S, SN, SP, st, keep("S", l))
-        Tr, TrN, TrP = rnd(T, TN, TP, st, keep("T", l))
-        W1r = br(W1) if keep("W1", l) else W1
-        W2r = br(W2) if keep("W2", l) else W2
+        Sr, SrN, SrP = rnd(S, SN, SP, st, keep_bf("S", l))
+        Tr, TrN, TrP = rnd(T, TN, TP, st, keep_bf("T", l))
+        W1r = br(W1) if keep_bf("W1", l) else W1
+        W2r = br(W2) if keep_bf("W2", l) else W2
         y1 = mm(Sr, SrN, SrP, W1r, Z(W1r), Z(W1r), True)
         y2 = mm(Tr, TrN, TrP, W2r, Z(W2r), Z(W2r), True)
         y = (y1[0] + b1) + (y2[0] + b2)
@@ -264,6 +312,9 @@ def ngcf_ref(E0, W, U, g, dims, bu, bi, bj, reg=(0.0, 0.0), tower_dtype=0, dt=F6
         st.add(unc)
         z = torch.where(y > 0, y, 0.2 * y)
         zN, zP = yN, yP
+        if mf is not None:                                          # Dropout: one more fp32 product per kept element
+            z = z * mf[l]
+            zN, zP = zN * _A(mf[l]) + _A(z), zP * _A(mf[l])
         rn = torch.clamp(torch.sqrt((z.to(F64) ** 2).sum(1)), min=1e-12)
         nv = z / rn.to(dt)[:, None]
         nA = _A(nv)
@@ -295,6 +346,9 @@ def ngcf_ref(E0, W, U, g, dims, bu, bi, bj, reg=(0.0, 0.0), tower_dtype=0, dt=F6
         dotP = (_A(dn) * a["nP"] + dnP * nA).sum(1, keepdim=True)
         dzN = (dnN + nA * dotN + a["nN"] * _A(dot)) / rn + _A(dz) * (a["rnN"][:, None] / rn + 1)
         dzP = (dnP + nA * dotP + a["nP"] * _A(dot)) / rn
+        if mf is not None and "msg_bwd_unmasked" not in defects:   # Dropout backward, on the fp32-rounded dz
+            dz = dz * mf[l]
+            dzN, dzP = dzN * _A(mf[l]) + _A(dz), dzP * _A(mf[l])
         y = a["y"]
         pos = (y < 0) if "leaky_wrong_side" in defects else (y > 0)
         slope = torch.where(pos, 1.0, 0.2).to(dt)
@@ -312,7 +366,7 @@ def ngcf_ref(E0, W, U, g, dims, bu, bi, bj, reg=(0.0, 0.0), tower_dtype=0, dt=F6
                 continue
             lo, hi = lay[l][nm]
             gW[lo:hi] += col; NW[lo:hi] += colN; PW[lo:hi] += colP
-        dYr, dYrN, dYrP = rnd(dY, dYN, dYP, st, keep("dY", l))
+        dYr, dYrN, dYrP = rnd(dY, dYN, dYP, st, keep_bf("dY", l))
         for A_, AN_, AP_, nm in ((a["Sr"], a["SrN"], a["SrP"], "W1"), (a["Tr"], a["TrN"], a["TrP"], "W2")):
             v, N_, P_ = mm(dYr.T.contiguous(), dYrN.T.contiguous(), dYrP.T.contiguous(), A_, AN_, AP_, False)
             lo, hi = lay[l][nm]
@@ -326,7 +380,8 @@ def ngcf_ref(E0, W, U, g, dims, bu, bi, bj, reg=(0.0, 0.0), tower_dtype=0, dt=F6
         dX = dS[0] + dT[0] * El
         dXN = dS[1] + _A(dT[0]) * ElN + dT[1] * _A(El) + _A(dT[0] * El) + _A(dX)
         dXP = dS[2] + _A(dT[0]) * ElP + dT[2] * _A(El)
-        AdX, AdXN, AdXP = spmm(g, dX, dt), spmm(g, _A(dX) + dXN, F64), spmm(g, dXP, F64)
+        gt = gl[l] if "node_bwd_untransposed" in defects else gl[l].T    # a defect: A_drop in place of A_drop^T
+        AdX, AdXN, AdXP = spmm(gt, dX, dt), spmm(gt, _A(dX) + dXN, F64), spmm(gt, dXP, F64)
         dE, dEN, dEP = dEl + AdX, dElN + AdXN + _A(dEl + AdX), dElP + AdXP
     gE = (dE + G[:, :dims[0]]).to(F64)
     NE = dEN + GN[:, :dims[0]] + _A(gE)
@@ -374,11 +429,13 @@ class _Graph:
         self.kappa = kappa_of("lgcn" if dims is None else "ngcf", td)
         self.ref_uses_kappa = dims is not None
 
-    def reference(self, pre, idx, kappa, dt=F64, defects=()):
+    def reference(self, pre, idx, kappa, dt=F64, defects=(), keep=None, p=0.0, edge=None, node_p=0.0, forward=None):
+        """keep, p, edge, node_p: one step's NGCF dropout masks (ngcf_ref); forward: the step's forward counter (the device's)"""
         if self.dims is None:
             res = lgcn_ref(pre["E0"], self.U, self.rg, self.L, *idx, self.reg, dt, defects)
             return dict(res, g=dict(E0=res["g"]), N=dict(E0=res["N"]), P=dict(E0=res["P"]))
-        res = ngcf_ref(pre["E0"], pre["W"], self.U, self.rg, self.dims, *idx, self.reg, self.td, dt, defects, kappa)
+        res = ngcf_ref(pre["E0"], pre["W"], self.U, self.rg, self.dims, *idx, self.reg, self.td, dt, defects, kappa, keep, p, edge,
+                       node_p)
         return dict(res, **{x: dict(E0=res[x][0], W=res[x][1]) for x in ("g", "N", "P")})
 
     def sections(self):
@@ -416,7 +473,8 @@ class Gpu(_Graph, Stepper):
             self.mom = {key: (v[m].view(self.t[key].shape), v[s].view(self.t[key].shape)) for key, (m, s) in moms.items()}
         torch.cuda.synchronize()
 
-    def run(self, lo, n, batch, k, adam_step0=0, apply=True, first_step=0):
+    def run(self, lo, n, batch, k, adam_step0=0, apply=True, first_step=0, **step):
+        assert not step, "steps without dropout (DropGpu of test_gpu_ngcf_dropout_fp64.py takes masks)"
         bu, bi, bj = (p[lo:lo + n] for p in self.planes)
         if self.dims is None:
             out = self.ops.lgcn_bpr_train_steps(self.t["E0"], self.ws, self.graph, self.L, bu, bi, bj, batch, first_step, k,
@@ -595,15 +653,17 @@ def test_lgcn_launches(gpu):
 
 
 # ---------------------------------------------------------------- GPU: NGCF
-def ngcf_forward_check(ops, graph, rg, U, I, E0, W, dims, td):
-    """ngcf_forward against the reference -> (worst error/bound at the module's KAPPA, smallest KAPPA of KAPPA_LADDER that
-    bounds every element)"""
-    ws = ops.NgcfWorkspace(U, I, dims, "sgd", "cuda")
-    got = ops.ngcf_forward(E0, W, ws, graph, tower_dtype=td).to(F64)
+def ngcf_forward_check(ops, graph, rg, U, I, E0, W, dims, td, keep=None, p=0.0, edge=None, node_p=0.0, got=None):
+    """ngcf_forward (or the device forward `got`, e.g. ngcf_forward_philox's) against the reference with the same masks ->
+    (worst error/bound at the module's KAPPA, smallest KAPPA of KAPPA_LADDER that bounds every element)"""
+    if got is None:
+        ws = ops.NgcfWorkspace(U, I, dims, "sgd", "cuda")
+        got = ops.ngcf_forward(E0, W, ws, graph, tower_dtype=td, dropout=p, keep=keep)
+    got = got.to(F64)
     z = torch.zeros(1, dtype=torch.long, device="cuda")
 
     def ratio(k):
-        res = ngcf_ref(E0, W, U, rg, dims, z, z, z, (0.0, 0.0), td, kappa=k)
+        res = ngcf_ref(E0, W, U, rg, dims, z, z, z, (0.0, 0.0), td, kappa=k, keep=keep, p=p, edge=edge, node_p=node_p)
         bound = k * U_RND * res["ALLN"] + res["ALLP"] + 2 * U_RND * res["ALL"].abs().to(F64)
         err = (got - res["ALL"].to(F64)).abs()
         return float(torch.where(err > 0, err / bound, torch.zeros_like(err)).max())
@@ -753,8 +813,8 @@ def test_reference_without_rounding_matches_oracle(orc, model, opt):
                 assert float(off.max()) > 100 * 2e-6 * max(1.0, float(np.abs(want).max()))
 
 
-def _cpu_case(model, seed=11, opt="sgd", reg=(1e-3, 1e-3), td=0, dims=(16, 12, 10), L=3, F=16, defects=(), big=False):
-    """a CPU problem with multi-segment rows; -> (stepper, graph, B)"""
+def _cpu_case(model, seed=11, opt="sgd", reg=(1e-3, 1e-3), td=0, dims=(16, 12, 10), L=3, F=16, defects=(), big=False, cls=None):
+    """a CPU problem with multi-segment rows; -> (stepper (a StandIn, or cls), graph, B)"""
     rng = np.random.default_rng(seed)
     U, I = (400, 300) if not big else (1200, 900)
     adj = random_graph(rng, U, I, 4000 if not big else 12000, zipf=1.1)
@@ -766,8 +826,8 @@ def _cpu_case(model, seed=11, opt="sgd", reg=(1e-3, 1e-3), td=0, dims=(16, 12, 1
     B = 700
     planes = planes_uniform(rng, U, I, 2 * B)
     lr = 0.05 if opt == "sgd" else 0.01
-    st = StandIn(rg, U, I, E0, W, planes, L if model == "lgcn" else len(dims) - 1, opt, lr, reg,
-                 None if model == "lgcn" else list(dims), td, defects)
+    st = (cls or StandIn)(rg, U, I, E0, W, planes, L if model == "lgcn" else len(dims) - 1, opt, lr, reg,
+                          None if model == "lgcn" else list(dims), td, defects)
     return st, rg, B
 
 

@@ -42,6 +42,8 @@ from fp64_step import (F64, GAMMA, U_RND, Flags, Stepper, _A, br, carve, checked
 # KAPPA_LADDER at which every element of the step passes; the ladder starts at 0.125.
 #   NFM fp32: 1.0 (geometry F = 6, L = 3, sigmoid; 0.35 on the launches, <= 0.125 at the bench shape), hence 2.
 #   NFM bf16: 1.0 (the launches; <= 0.5 elsewhere), hence 2.
+#   NFM with dropout_engine 'philox' (test_nfm_philox_dropout, p = 0.5, the hook's masks): fp32 0.005, worst error/bound
+#     0.49; bf16 0.5 (ladder), worst error/bound 1.00, at most 33 % of the intermediates flagged.
 #   FM: 1.94 (HL under SGD, P[2223, 44]; 1.69 at the bench shape under SGD), hence 4.
 # Power (test_harness_power_in_every_gpu_configuration): in every (bn, L, act) a GPU case runs, a 1e-3 relative gradient error
 # (5e-3 in bf16) in P, W0, wp or BN0's gamma and each bf16 operand left unrounded exceed the bound.  The defective stand-ins
@@ -603,6 +605,20 @@ class NfmGpu(_Gpu):
         return out.cpu().numpy()
 
 
+class NfmPhiloxGpu(NfmGpu):
+    """NFM steps with dropout_engine 'philox': the masks are drawn on the device, step s keyed by (seed, adam_step0 + s); the
+    reference takes the same masks as bytes from ops.nfm_philox_masks (run ignores them)"""
+    seed = 0
+
+    def run(self, lo, n, batch, k, adam_step0=0, apply=True, first_step=0, keep=None):
+        bu, bi, bj = (p[lo:lo + n] for p in self.planes)
+        out = self.ops.nfm_bpr_train_steps_philox(self.P, self.Q, self.bias, self.N, self.Rs if self.bn else None, self.ws,
+                                                  self.act, bu, bi, bj, batch, first_step, k, self.hp, adam_step0=adam_step0,
+                                                  apply=apply, tower_dtype=self.td, dropout=self.dropout, seed=self.seed)
+        torch.cuda.synchronize()
+        return out.cpu().numpy()
+
+
 class FmGpu(_Gpu):
     def __init__(self, U, I, P, Q, bias, planes, loss, opt, lr, reg):
         from daisyrec_b200 import _lib, ops
@@ -684,7 +700,7 @@ def gpu():
 
 
 # ---------------------------------------------------------------- GPU: NFM
-def _nfm_bench(opt, td, dropout=0.0, seed=11, nsteps=3, lr=None):
+def _nfm_bench(opt, td, dropout=0.0, seed=11, nsteps=3, lr=None, cls=NfmGpu):
     from daisyrec_b200.utils.synthetic import init_tables
     U, I = ml20m()
     F, L, B = 64, 1, 1 << 18
@@ -695,8 +711,7 @@ def _nfm_bench(opt, td, dropout=0.0, seed=11, nsteps=3, lr=None):
     N, Rs = nfm_net(F, L, True, g)
     planes = uniform_planes(g, U, I, nsteps * B)
     lr0, reg = (0.001, (0.0, 0.001)) if opt == "adam" else (0.05, (1e-3, 1e-3))
-    st = NfmGpu(U, I, P, Q, bias, N, Rs, planes, L, True, 0, opt, lr or lr0, reg, td, max_rows=2 * B,
-                dropout=dropout)
+    st = cls(U, I, P, Q, bias, N, Rs, planes, L, True, 0, opt, lr or lr0, reg, td, max_rows=2 * B, dropout=dropout)
     return st, B, g
 
 
@@ -729,6 +744,19 @@ def test_nfm_default_dropout(gpu, td):
     for s, (_, res) in enumerate(out):
         assert abs(float(l3[s]) - res["loss"]) <= kappa_of("nfm", td) * U_RND * res["lossN"] + res["lossP"], (s, l3[s], res["loss"])
     report(f"nfm dropout td={td}", recs)
+
+
+@pytest.mark.gpu
+@pytest.mark.parametrize("td", [0, 1])
+def test_nfm_philox_dropout(gpu, td):
+    """p = 0.5 at the bench shape with dropout_engine 'philox': three teacher-forced steps at global steps 4, 5, 6, each
+    against nfm_ref with the keep factors of ops.nfm_philox_masks at that step (the kernels' own nfm_keep_factor)"""
+    ops = gpu
+    st, B, g = _nfm_bench("sgd", td, dropout=0.5, seed=25, lr=0.002, cls=NfmPhiloxGpu)
+    st.seed = 0x5EED + td
+    recs = [checked_step(st, s * B, B, B, f"philox td={td} step {4 + s}", adam_step0=4 + s, ref_device="cuda",
+                         keep=ops.nfm_philox_masks(st.seed, 4 + s, B, st.F, st.L, 0.5, "cuda")) for s in range(3)]
+    report(f"nfm philox dropout td={td}", recs)
 
 
 # (F, L, act, bn, B): every F in NFM_F, L in NFM_L, activation, BatchNorm on and off and B in NFM_B at least once.  BatchNorm
