@@ -42,8 +42,16 @@ inline int pick_tile(long long per_cta, int cap = kTileDefault)
 #endif
 
 // ------------------------------------------------------------------ device pieces
-// deterministic mode: contribution -> 2^40 fixed point (|sum| < 8.3e6, resolution 9e-13), scalars -> 2^24
-constexpr double kDetScale = 1099511627776.0, kDetAccScale = 16777216.0;
+// deterministic mode: contribution -> 2^40 fixed point (|sum| < 2^23 = 8.4e6, resolution 9e-13).  The step's scalar sums, each
+// lane's share of one triple rounded on its own (that share depends on the row geometry alone, so the integer totals do not
+// depend on how triples map to threads: tile size, grid, SM count): the loss -> 2^24 (|sum| < 2^39 = 5.5e11, resolution 6e-8),
+// the l1 and squared-norm sums of the batch rows -> 2^32 (|sum| < 2^31 = 2.1e9, resolution 2.3e-10: the batch norms, and
+// through them the reg_2 term, stay as close to fp64 as the fp32 partials were).  No range bounds what a diverging run reaches
+// (SL's (x - y)^2 and HL's margin are unbounded), so every value and every integer addition is checked: a non-finite value,
+// one of 2^62 units or more, or an addition that overflows int64 makes the step report a non-finite loss (DRB_ERR_NAN_LOSS)
+// before phase 2 applies it.
+constexpr double kDetScale = 1099511627776.0, kDetAccScale = 16777216.0, kDetNormScale = 4294967296.0;
+constexpr double kDetValueMax = 4611686018427387904.0;   // 2^62
 
 __device__ __forceinline__ float sgnf(float x) { return (float)((x > 0.f) - (x < 0.f)); }
 
@@ -276,9 +284,30 @@ __device__ __forceinline__ int draw_negative(const StepParams &p, int u, unsigne
 template <bool LEAN> struct RowOffset { typedef size_t type; };
 template <> struct RowOffset<true> { typedef unsigned type; };
 
-__device__ __forceinline__ void det_red(long long *p, float v)
+// deterministic mode: a + b in int64; ok becomes false when the sum overflows
+__device__ __forceinline__ long long det_add(long long a, long long b, bool &ok)
 {
-    red_add_u64(reinterpret_cast<unsigned long long *>(p), (unsigned long long)__double2ll_rn((double)v * kDetScale));
+    const long long s = (long long)((unsigned long long)a + (unsigned long long)b);
+    ok = ok && ((a ^ s) & (b ^ s)) >= 0;
+    return s;
+}
+
+// deterministic mode: v in `scale` fixed point; ok becomes false for a non-finite value or one of 2^62 units or more
+__device__ __forceinline__ long long det_fix(float v, double scale, bool &ok)
+{
+    const double s = (double)v * scale;
+    if (!(fabs(s) < kDetValueMax)) { ok = false; return 0; }
+    return __double2ll_rn(s);
+}
+
+// deterministic mode: add one contribution to a table element's fixed-point sum; the returned old value shows an overflow of
+// the sum.  A sum whose final value leaves the int64 range crosses it in every order of the additions, so it is always seen.
+__device__ __forceinline__ void det_red(long long *p, float v, bool &ok)
+{
+    const long long x = det_fix(v, kDetScale, ok);
+    if (x == 0) return;
+    const long long old = (long long)atomicAdd(reinterpret_cast<unsigned long long *>(p), (unsigned long long)x);
+    det_add(old, x, ok);
 }
 
 // Exchange policy of the single-GPU kernel: nothing to exchange (every hook is a compile-time no-op).
@@ -324,7 +353,11 @@ __device__ __forceinline__ void bpr_steps_body(StepParams &p, XCH &xch)
     // index tiles: three planes u, i, j; UBK: kTileMax (u, i, j, 0) records
     __shared__ __align__(128) int32_t s_idx[2][UBK ? 4 : 3][kTileMax];
     __shared__ uint64_t s_bar[2];
-    __shared__ double s_red[8][kThreads / 32];
+    __shared__ union {
+        double d[8][kThreads / 32];
+        long long i[8][kThreads / 32];   // GEN && det: the fixed-point partials
+    } s_red_u;
+    double (&s_red)[8][kThreads / 32] = s_red_u.d;
     extern __shared__ __align__(16) unsigned char s_dyn[];   // UBK: partition histogram, then (staged rows +) bucket accumulator
     __shared__ int s_claim[3];                               // UBK: claimed bucket, its first and end position
     __shared__ unsigned s_wsum[kThreads / 32];               // UBK: per-warp sums of the bucket-count scan
@@ -433,7 +466,10 @@ __device__ __forceinline__ void bpr_steps_body(StepParams &p, XCH &xch)
 
         // ------------------------------------------------------------ phase 1
         if (p.phases & 1) {
-        if (tid < 8 * (kThreads / 32)) (&s_red[0][0])[tid] = 0.0;   // per-warp fp64 accumulators of this step
+        if (tid < 8 * (kThreads / 32)) {   // per-warp fp64 (GEN && det: int64) accumulators of this step
+            if (GEN && p.det) (&s_red_u.i[0][0])[tid] = 0; else (&s_red[0][0])[tid] = 0.0;
+        }
+        bool det_ok = true;   // GEN && det: every value and addition of this step's fixed-point sums was in range
         __syncthreads();
         int buf = 0;
         long long t_i = blockIdx.x;
@@ -575,6 +611,10 @@ __device__ __forceinline__ void bpr_steps_body(StepParams &p, XCH &xch)
             constexpr int XS = UBK ? 4 : 1;
             const int32_t *xu = s_idx[buf][0], *xi = UBK ? xu + 1 : s_idx[buf][1], *xj = UBK ? xu + 2 : s_idx[buf][2];
             float t_loss = 0.f, t_l1u = 0.f, t_l1i = 0.f, t_l1j = 0.f, t_s2u = 0.f, t_s2i = 0.f, t_s2j = 0.f, t_gb0 = 0.f;
+            long long x_fx[7] = {0, 0, 0, 0, 0, 0, 0};   // GEN && det: the same seven sums, per triple in fixed point (det_acc)
+            auto det_acc = [&](int k, float v) {
+                x_fx[k] = det_add(x_fx[k], det_fix(v, k == 0 ? kDetAccScale : kDetNormScale, det_ok), det_ok);
+            };
             // UBK + ustage: the tile's records are counting-sorted by local user into s_perm (user ul's run is
             // s_perm[s_uoff[ul] .. s_uoff[ul + 1])), and group g walks the sorted positions [lo, hi) = [g span, (g + 1) span), UNR
             // consecutive ones at a time.  It sums the user gradient of a run in registers (ua) and adds it to s_gp when the user
@@ -758,7 +798,9 @@ __device__ __forceinline__ void bpr_steps_body(StepParams &p, XCH &xch)
                         if ((gl % UNR) == r) { p_own = ps[r]; n_own = ns[r]; ok_own = ok[r]; }
                     float cp_own, cn_own;
                     const float l_own = pair_loss(p_own, n_own, cp_own, cn_own);
-                    if (gl < UNR && ok_own) t_loss += l_own;
+                    if (gl < UNR && ok_own) {
+                        if (GEN && p.det) det_acc(0, l_own); else t_loss += l_own;
+                    }
 #pragma unroll
                     for (int r = 0; r < UNR; ++r) {
                         cs[r] = __shfl_sync(0xffffffffu, cp_own, (lane - gl) + r);
@@ -768,7 +810,9 @@ __device__ __forceinline__ void bpr_steps_body(StepParams &p, XCH &xch)
 #pragma unroll
                     for (int r = 0; r < UNR; ++r) {
                         const float l = pair_loss(ps[r], ns[r], cs[r], cn[r]);
-                        if (gl == 0 && ok[r]) t_loss += l;
+                        if (gl == 0 && ok[r]) {
+                            if (GEN && p.det) det_acc(0, l); else t_loss += l;
+                        }
                     }
                 }
 #pragma unroll
@@ -792,9 +836,14 @@ __device__ __forceinline__ void bpr_steps_body(StepParams &p, XCH &xch)
                                 l1i += fabsf(b); s2i = fmaf(b, b, s2i);
                                 l1j += fabsf(d); s2j = fmaf(d, d, s2j);
                             }
-                        t_l1u += l1u; t_s2u += s2u;
-                        t_l1i += l1i; t_l1j += l1j;
-                        t_s2i += s2i; t_s2j += s2j;
+                        if (GEN && p.det) {
+                            det_acc(1, l1u); det_acc(2, l1i); det_acc(3, l1j);
+                            det_acc(4, s2u); det_acc(5, s2i); det_acc(6, s2j);
+                        } else {
+                            t_l1u += l1u; t_s2u += s2u;
+                            t_l1i += l1i; t_l1j += l1j;
+                            t_s2i += s2i; t_s2j += s2j;
+                        }
                     }
                     if (p.apply) {
                         if constexpr (UBK && STAGED) {
@@ -831,9 +880,9 @@ __device__ __forceinline__ void bpr_steps_body(StepParams &p, XCH &xch)
                             if (GEN && p.det) {
 #pragma unroll
                                 for (int e = 0; e < VEC; ++e) {
-                                    det_red(p.ws.gP64 + ou[r] + cc * VEC + e, gu.v[e]);
-                                    det_red(p.ws.gQ64 + oi[r] + cc * VEC + e, gi.v[e]);
-                                    if (!pw) det_red(p.ws.gQ64 + oj[r] + cc * VEC + e, gj.v[e]);
+                                    det_red(p.ws.gP64 + ou[r] + cc * VEC + e, gu.v[e], det_ok);
+                                    det_red(p.ws.gQ64 + oi[r] + cc * VEC + e, gi.v[e], det_ok);
+                                    if (!pw) det_red(p.ws.gQ64 + oj[r] + cc * VEC + e, gj.v[e], det_ok);
                                 }
                             } else {
                                 if constexpr (UBK && STAGED) {
@@ -876,11 +925,19 @@ __device__ __forceinline__ void bpr_steps_body(StepParams &p, XCH &xch)
             }
             if constexpr (UBK && STAGED) flush();
             // per-thread fp32 partials cover <= tile/GROUPS triples: warp-reduce, widen to fp64 in smem
+            // (GEN && det: the fixed-point partials are summed as integers, in the same smem slots; FM's biases never run det)
             {
                 float tv[8] = {t_loss, t_l1u, t_l1i, t_l1j, t_s2u, t_s2i, t_s2j, t_gb0};
                 const int nv = has_reg ? 7 : 1;
                 for (int k = 0; k < 8; ++k) {
                     if (k >= nv && !(GEN && k == 7 && p.bias != nullptr)) continue;
+                    if (GEN && p.det && k < 7) {
+                        long long v = x_fx[k];
+#pragma unroll
+                        for (int off = 16; off >= 1; off >>= 1) v = det_add(v, __shfl_xor_sync(0xffffffffu, v, off), det_ok);
+                        if (lane == 0) s_red_u.i[k][warp] = det_add(s_red_u.i[k][warp], v, det_ok);
+                        continue;
+                    }
                     float v = tv[k];
 #pragma unroll
                     for (int off = 16; off >= 1; off >>= 1) v += __shfl_xor_sync(0xffffffffu, v, off);
@@ -934,26 +991,39 @@ __device__ __forceinline__ void bpr_steps_body(StepParams &p, XCH &xch)
         // CTA reduction of the 7 partial sums -> one fp64 atomic each
         __syncthreads();
         if (tid < (has_reg ? 7 : 1) || (GEN && tid == 7 && p.bias != nullptr)) {
-            double v = 0;
-            for (int w = 0; w < kThreads / 32; ++w) v += s_red[tid][w];
             if (GEN && p.det) {
-                if (v != 0.0) red_add_u64(reinterpret_cast<unsigned long long *>(p.ws.accfx + tid),
-                                          (unsigned long long)__double2ll_rn(v * kDetAccScale));
-            } else if (v != 0.0) {
-                atomicAdd(&acc[tid], v);
+                long long v = 0;
+                for (int w = 0; w < kThreads / 32; ++w) v = det_add(v, s_red_u.i[tid][w], det_ok);
+                if (v != 0) {
+                    const long long old = (long long)atomicAdd(reinterpret_cast<unsigned long long *>(p.ws.accfx + tid),
+                                                               (unsigned long long)v);
+                    det_add(old, v, det_ok);
+                }
+            } else {
+                double v = 0;
+                for (int w = 0; w < kThreads / 32; ++w) v += s_red[tid][w];
+                if (v != 0.0) atomicAdd(&acc[tid], v);
             }
         }
+        // GEN && det: a value or sum out of range anywhere in the CTA flags the step in accfx[7] (a slot FM's bias sum would use;
+        // FM never runs det), read back before phase 2
+        if (GEN && p.det)
+            if (!__syncthreads_and(det_ok) && tid == 0) red_add_u64(reinterpret_cast<unsigned long long *>(p.ws.accfx + 7), 1ull);
         }  // phase 1
         if (p.phases == 3) grid_barrier(&hdr->barrier, epoch);
         if constexpr (UBK)
             if (blockIdx.x == 0 && tid == 0) p.ub_count[2 * p.ub_buckets] = 0u;   // every claim of this step is done
         if (!(p.phases & 2)) break;   // split mode: the host reduces gQ / counters / acc across ranks now
         if (GEN && p.det) {
-            // fixed-point scalar sums -> acc (the table sums stay in fixed point: the DET sweep reads and clears them)
-            const long long gt = (long long)blockIdx.x * kThreads + tid;
-            if (gt < 8) {
-                acc[gt] = (double)__ldcg(p.ws.accfx + gt) / kDetAccScale;
-                __stcg(p.ws.accfx + gt, 0ll);
+            // fixed-point scalar sums -> acc (the table sums stay in fixed point: the DET sweep reads and clears them); a flagged
+            // step gets a NaN loss, which every CTA sees after the barrier and which stops the launch before phase 2
+            if (blockIdx.x == 0 && tid == 0) {
+                const bool flagged = __ldcg(p.ws.accfx + 7) != 0;
+                for (int k = 0; k < 8; ++k) {
+                    acc[k] = (k == 0 && flagged) ? __longlong_as_double(0x7ff8000000000000ll)
+                                                 : (double)__ldcg(p.ws.accfx + k) / (k == 0 ? kDetAccScale : kDetNormScale);
+                    __stcg(p.ws.accfx + k, 0ll);
+                }
             }
             grid_barrier(&hdr->barrier, epoch);
         }
