@@ -645,6 +645,18 @@ extern "C" int drb_mf_last_step_mode(void) { return drb::g_last_step_mode; }
 // bucket width)
 extern "C" int drb_mf_last_step_staged(void) { return drb::g_last_step_staged; }
 
+#ifdef DRB_PHASE_TIMERS
+// probe build only: the phase timers of the last staged launch (u64 [kPtSteps][kPtMarks][kPtCtas]) into `dst`, and their
+// dimensions into dims[3]
+extern "C" int drb_phase_timers(void *dst, int32_t *dims)
+{
+    dims[0] = drb::kPtSteps; dims[1] = drb::kPtMarks; dims[2] = drb::kPtCtas;
+    DRB_CUDA(cudaDeviceSynchronize());
+    DRB_CUDA(cudaMemcpyFromSymbol(dst, drb::g_phase_t, sizeof(drb::g_phase_t)));
+    return DRB_OK;
+}
+#endif
+
 // the timing half of the on-device selection for `factors`: milliseconds of the timed launch (3 steps of 524 288 triples) of the
 // general instantiation and of the best lean candidate, and the index-tile cap in use (runs the selection if it has not run)
 extern "C" int drb_mf_step_selfcheck_ms(int32_t F, int64_t table_rows, float *ms_general, float *ms_lean, int32_t *tile_cap)

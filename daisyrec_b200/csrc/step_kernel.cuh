@@ -41,6 +41,24 @@ inline int pick_tile(long long per_cta, int cap = kTileDefault)
 #define DRB_UNR 2              // triples in flight per lane group (memory-level parallelism)
 #endif
 
+// Phase timers of the staged user-bucketed form, compiled in only by the probe build (-DDRB_PHASE_TIMERS,
+// scripts/probe_mf_phases.py --timers): thread 0 of every CTA writes %globaltimer at each phase boundary of the first
+// kPtSteps steps of a launch into g_phase_t[step][mark][cta]; drb_phase_timers (mf_bpr.cu) copies it to the host.
+#ifdef DRB_PHASE_TIMERS
+constexpr int kPtSteps = 96, kPtMarks = 12, kPtCtas = 512;
+__device__ unsigned long long g_phase_t[kPtSteps][kPtMarks][kPtCtas];
+__device__ __forceinline__ void phase_mark(long long s, int m)
+{
+    if (threadIdx.x == 0 && s < kPtSteps && blockIdx.x < kPtCtas) {
+        unsigned long long t;
+        asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t)::"memory");
+        g_phase_t[s][m][blockIdx.x] = t;
+    }
+}
+#else
+__device__ __forceinline__ void phase_mark(long long, int) {}
+#endif
+
 // ------------------------------------------------------------------ device pieces
 // deterministic mode: contribution -> 2^40 fixed point (|sum| < 2^23 = 8.4e6, resolution 9e-13).  The step's scalar sums, each
 // lane's share of one triple rounded on its own (that share depends on the row geometry alone, so the integer totals do not
@@ -441,6 +459,8 @@ __device__ __forceinline__ void bpr_steps_body(StepParams &p, XCH &xch)
     // UBK + SGD with the norm cache: user rows staged and updated per bucket (see above); unorm: the cache is kept (regulariser on)
     constexpr bool ustage = UBK && STAGED;
     const bool unorm = ustage && ((p.reg1 != 0.f) || (p.reg2 != 0.f));
+    auto mark = [&](long long s, int m) { if constexpr (ustage) phase_mark(s, m); };
+    mark(0, 9);
     if constexpr (UBK) {
         if (unorm) {   // fill the norm cache: one pass over P and Q per launch (the item rows' entries follow the users')
             const long long nu = (long long)p.U * (W * NCH), nt = nu + (long long)p.I * (W * NCH);
@@ -451,7 +471,9 @@ __device__ __forceinline__ void bpr_steps_body(StepParams &p, XCH &xch)
                 const float2 n = row_norms<W * NCH>(v);
                 if (k < nt && k % (W * NCH) == 0) p.ub_norm[k / (W * NCH)] = n;
             }
+            mark(0, 10);
             grid_barrier(&hdr->barrier, epoch);
+            mark(0, 11);
         }
     }
 
@@ -463,6 +485,7 @@ __device__ __forceinline__ void bpr_steps_body(StepParams &p, XCH &xch)
         double *acc = hdr->acc[s & 1];
         const bool has_reg = (p.reg1 != 0.f) || (p.reg2 != 0.f);
         if constexpr (XCH::kActive) xch.begin_step(p, s, acc);   // item-side accumulators of this step's parity
+        mark(s, 0);
 
         // ------------------------------------------------------------ phase 1
         if (p.phases & 1) {
@@ -490,14 +513,29 @@ __device__ __forceinline__ void bpr_steps_body(StepParams &p, XCH &xch)
             for (int b = tid; b < NBK; b += kThreads) s_hist[b] = 0u;
             __syncthreads();
             const long long g0 = (long long)blockIdx.x * kThreads + tid, gstride = (long long)gridDim.x * kThreads;
+            // the partition's passes take PB of a thread's triples at a time and issue all their global loads before using any:
+            // one loop trip per triple waited out one round trip to L2 or HBM each (the norm-cache gathers are random).  The
+            // thread's triples are still summed and placed in the order t, t + gstride, ...
+            constexpr int PB = 4;
             float h_s2 = 0.f, h_l1 = 0.f;   // unorm: this thread's share of the batch's user norms, from the norm cache
-            for (long long t = g0; t < nb; t += gstride) {
-                const int u = __ldg(p.bu + base + t);
-                atomicAdd(&s_hist[u / UBU], 1u);
-                if (unorm) {
-                    const float2 n = __ldcg(p.ub_norm + u);
-                    h_s2 += n.x;
-                    h_l1 += n.y;
+            for (long long t0 = g0; t0 < nb; t0 += PB * gstride) {
+                int u[PB];
+                float2 n[PB];
+#pragma unroll
+                for (int q = 0; q < PB; ++q) {
+                    const long long t = t0 + q * gstride;
+                    u[q] = t < nb ? __ldg(p.bu + base + t) : -1;
+                }
+#pragma unroll
+                for (int q = 0; q < PB; ++q) n[q] = (unorm && u[q] >= 0) ? __ldcg(p.ub_norm + u[q]) : make_float2(0.f, 0.f);
+#pragma unroll
+                for (int q = 0; q < PB; ++q) {
+                    if (u[q] < 0) continue;
+                    atomicAdd(&s_hist[u[q] / UBU], 1u);
+                    if (unorm) {
+                        h_s2 += n[q].x;
+                        h_l1 += n[q].y;
+                    }
                 }
             }
             if (unorm) {
@@ -516,12 +554,35 @@ __device__ __forceinline__ void bpr_steps_body(StepParams &p, XCH &xch)
                 for (int w = 0; w < kThreads / 32; ++w) { v += s_red[tid][w]; s_red[tid][w] = 0.0; }
                 if (v != 0.0) atomicAdd(&acc[tid], v);
             }
+            mark(s, 1);
             grid_barrier(&hdr->barrier, epoch);
-            // exclusive scan of the counts in every CTA; CTA 0 publishes the ranges; each CTA reserves its slice of every bucket
-            // it holds triples of
+            mark(s, 2);
+            // each CTA reserves its slice of every bucket it holds triples of (s_hist becomes the slice's start within the bucket)
+            // and copies the counts into s_off; eight buckets per thread at a time, their count loads and reservation atomics in
+            // flight together.  Then an exclusive scan of the counts in every CTA; CTA 0 publishes the ranges.
+            for (int bb = tid; bb < NBK; bb += 8 * kThreads) {
+                unsigned c[8], r[8];
+#pragma unroll
+                for (int q = 0; q < 8; ++q) {
+                    const int b = bb + q * kThreads;
+                    c[q] = 0u;
+                    r[q] = 0u;
+                    if (b < NBK) {
+                        c[q] = __ldcg(ucnt + b);
+                        const unsigned h = s_hist[b];
+                        if (h != 0u) r[q] = atomicAdd(ucur + b, h);
+                    }
+                }
+#pragma unroll
+                for (int q = 0; q < 8; ++q) {
+                    const int b = bb + q * kThreads;
+                    if (b < NBK) { s_off[b] = c[q]; s_hist[b] = r[q]; }
+                }
+            }
+            __syncthreads();
             const int per = (NBK + kThreads - 1) / kThreads, b0 = min(NBK, tid * per), b1 = min(NBK, b0 + per);
             unsigned run = 0u;
-            for (int b = b0; b < b1; ++b) run += __ldcg(ucnt + b);
+            for (int b = b0; b < b1; ++b) run += s_off[b];
             unsigned incl = run;
 #pragma unroll
             for (int off = 1; off < 32; off <<= 1) {
@@ -533,25 +594,42 @@ __device__ __forceinline__ void bpr_steps_body(StepParams &p, XCH &xch)
             unsigned start = incl - run;
             for (int w = 0; w < warp; ++w) start += s_wsum[w];
             for (int b = b0; b < b1; ++b) {
-                const unsigned c = __ldcg(ucnt + b), h = s_hist[b];
+                const unsigned c = s_off[b];
                 if (blockIdx.x == 0) { p.ub_range[2 * b] = (int)start; p.ub_range[2 * b + 1] = (int)(start + c); }
-                s_off[b] = h != 0u ? start + atomicAdd(ucur + b, h) : 0u;
+                s_off[b] = start + s_hist[b];
                 s_hist[b] = 0u;
                 start += c;
             }
             __syncthreads();
+            mark(s, 3);
             // ---- scatter this CTA's triples into the partitioned records (the same triples as the histogram pass); a CTA holds
             // about two triples per bucket, so these stores land at random: one 16-byte store per triple, not three 4-byte ones
             // unorm: this pass also sums the item rows' cached norms over the batch (l1i, l1j, s2i, s2j)
             float h_in[4] = {0.f, 0.f, 0.f, 0.f};
-            for (long long t = g0; t < nb; t += gstride) {
-                const int u = __ldg(p.bu + base + t), b = u / UBU;
-                const int i = __ldg(p.bi + base + t), j = __ldg(p.bj + base + t);
-                const unsigned pos = s_off[b] + atomicAdd(&s_hist[b], 1u);
-                p.ub_t[pos] = make_int4(u, i, j, 0);
-                if (unorm) {
-                    const float2 ni = __ldcg(p.ub_norm + p.U + i), nj = __ldcg(p.ub_norm + p.U + j);
-                    h_in[0] += ni.y; h_in[1] += nj.y; h_in[2] += ni.x; h_in[3] += nj.x;
+            for (long long t0 = g0; t0 < nb; t0 += PB * gstride) {
+                int u[PB], i[PB], j[PB];
+                float2 ni[PB], nj[PB];
+#pragma unroll
+                for (int q = 0; q < PB; ++q) {
+                    const long long t = t0 + q * gstride;
+                    const bool ok = t < nb;
+                    u[q] = ok ? __ldg(p.bu + base + t) : -1;
+                    i[q] = ok ? __ldg(p.bi + base + t) : 0;
+                    j[q] = ok ? __ldg(p.bj + base + t) : 0;
+                }
+#pragma unroll
+                for (int q = 0; q < PB; ++q) {
+                    const bool g = unorm && u[q] >= 0;
+                    ni[q] = g ? __ldcg(p.ub_norm + p.U + i[q]) : make_float2(0.f, 0.f);
+                    nj[q] = g ? __ldcg(p.ub_norm + p.U + j[q]) : make_float2(0.f, 0.f);
+                }
+#pragma unroll
+                for (int q = 0; q < PB; ++q) {
+                    if (u[q] < 0) continue;
+                    const int b = u[q] / UBU;
+                    const unsigned pos = s_off[b] + atomicAdd(&s_hist[b], 1u);
+                    p.ub_t[pos] = make_int4(u[q], i[q], j[q], 0);
+                    if (unorm) { h_in[0] += ni[q].y; h_in[1] += nj[q].y; h_in[2] += ni[q].x; h_in[3] += nj[q].x; }
                 }
             }
             if (unorm) {
@@ -570,8 +648,10 @@ __device__ __forceinline__ void bpr_steps_body(StepParams &p, XCH &xch)
                 }
             }
             asm volatile("fence.proxy.async.global;" ::: "memory");   // the records are read back by bulk copies (async proxy)
+            mark(s, 4);
             grid_barrier(&hdr->barrier, epoch);
             for (long long k = g0; k < 2LL * NBK; k += gstride) ucnt[k] = 0u;   // counts, cursors: zero for the next step
+            mark(s, 5);
             // ustage: two slots of UBU staged user rows (the current bucket's and the next one's) before the accumulator
             s_rows = reinterpret_cast<float *>(s_dyn);
             s_gp = s_rows + (ustage ? 2 * UBU * F : 0);
@@ -1010,7 +1090,9 @@ __device__ __forceinline__ void bpr_steps_body(StepParams &p, XCH &xch)
         if (GEN && p.det)
             if (!__syncthreads_and(det_ok) && tid == 0) red_add_u64(reinterpret_cast<unsigned long long *>(p.ws.accfx + 7), 1ull);
         }  // phase 1
+        mark(s, 6);
         if (p.phases == 3) grid_barrier(&hdr->barrier, epoch);
+        mark(s, 7);
         if constexpr (UBK)
             if (blockIdx.x == 0 && tid == 0) p.ub_count[2 * p.ub_buckets] = 0u;   // every claim of this step is done
         if (!(p.phases & 2)) break;   // split mode: the host reduces gQ / counters / acc across ranks now
@@ -1197,6 +1279,7 @@ __device__ __forceinline__ void bpr_steps_body(StepParams &p, XCH &xch)
                 if (k != nbias - 1 && g != 0.f) __stcg(p.ws.gB + k, 0.f);
             }
         }
+        mark(s, 8);
         if constexpr (XCH::kActive) {
             if (!xch.end_step(p, s, epoch)) break;   // every rank's item slice has landed in this rank's replica
         } else {

@@ -7,12 +7,19 @@ Prints one JSON line per measurement (ms per step, CUDA events around launches t
   loss_only     ops.mf_bpr_loss: phase 1 without any RED (loads and loss only), one launch per step
   fused_sorted  the fused launch on planes sorted by user within each step (same batches, other fp32 summation order)
 and a first line with the card, its power limit and SM clocks.  Usage: python scripts/probe_mf_phases.py [steps] [reps]
+
+With --timers it instead builds the step library once more with -DDRB_PHASE_TIMERS (as scripts/build_variants.sh builds its
+A/B variants: mf_bpr.cu alone, linked with the other objects of the library build, into daisyrec_b200/lib/variants/), runs one
+fused launch of `steps` steps on it, and prints per section of the staged user-bucketed step the median over steps of the
+maximum over CTAs (ms), and of the time between the last CTAs to reach its two boundaries (the critical path).
 """
 import ctypes as C
 import json
 import os
 import subprocess
 import sys
+
+import numpy as np
 
 import torch
 
@@ -33,6 +40,77 @@ def card():
     except Exception as e:  # noqa: BLE001
         out = repr(e)
     return dict(zip(q.split(","), [x.strip() for x in out.split(",")]))
+
+
+# boundaries written by phase_mark (step_kernel.cuh), per step: 0 step start, 1 histogram done, 2 after its barrier, 3 scan and
+# reservation done, 4 scatter done, 5 after its barrier and the count zeroing, 6 phase 1 done, 7 after its barrier, 8 item sweep
+# done; launch start (9), norm-cache fill done (10) and after its barrier (11) in step 0's slots
+SECTIONS = (("histogram", 0, 1), ("barrier_hist", 1, 2), ("scan_reserve", 2, 3), ("scatter", 3, 4), ("barrier_scatter", 4, 5),
+            ("phase1", 5, 6), ("barrier_phase1", 6, 7), ("item_sweep", 7, 8), ("barrier_step", 8, None))
+
+
+def timer_lib():
+    """the probe build of the library (rebuilt when mf_bpr.cu or a header is newer)"""
+    from daisyrec_b200 import _build
+    out = os.path.join(_build.LIBDIR, "variants")
+    so = os.path.join(out, "lib_phase_timers.so")
+    if not _build._stale(so, [os.path.join(_build.CSRC, f) for f in os.listdir(_build.CSRC)]):
+        return so
+    _build.build()
+    os.makedirs(out, exist_ok=True)
+    obj = os.path.join(out, "mf_bpr_phase_timers.o")
+    subprocess.check_call([_build.nvcc()] + _build.ARCH + _build.FLAGS + ["-DDRB_PHASE_TIMERS", "-c",
+                          os.path.join(_build.CSRC, "mf_bpr.cu"), "-o", obj])
+    others = [os.path.join(_build.LIBDIR, f.replace(".cu", ".o")) for f in _build.SOURCES if f != "mf_bpr.cu"]
+    subprocess.check_call([_build.nvcc()] + _build.ARCH + ["-shared", "-cudart", "static", "-o", so, obj] + others + ["-ldl"])
+    os.remove(obj)
+    return so
+
+
+def phase_timers(K):
+    dev = torch.device("cuda", 0)
+    torch.cuda.set_device(dev)
+    seed, B, F = 2022, 1 << 20, 64
+    d, triples = bench.build_workload("ml-20m", dev, 4, seed, "cuda")
+    U, I = d["user_num"], d["item_num"]
+    g = torch.Generator(device=dev)
+    g.manual_seed(seed)
+    perm = torch.randperm(triples.shape[0], generator=g, device=dev)
+    bu, bi, bj = ops.gather_triples(triples, perm)
+    del perm, triples
+    bu, bi, bj = bu[:K * B].contiguous(), bi[:K * B].contiguous(), bj[:K * B].contiguous()
+    hp = ops.hyper(**bench.HYPER)
+    P, Q = init_tables(U, I, F, seed, dev)
+    ws = ops.MFWorkspace(U, I, F, "sgd", dev)
+    ops.mf_bpr_train_steps(P, Q, ws, bu, bi, bj, B, 0, 2, hp, check=False)            # warm-up
+    ops.mf_bpr_train_steps(P, Q, ws, bu, bi, bj, B, 0, K, hp, check=False)
+    torch.cuda.synchronize()
+    lib = L.lib()
+    assert lib.drb_mf_last_step_mode() == 2 and lib.drb_mf_last_step_staged() == 1, "the launch did not run the staged form"
+    dims = (C.c_int32 * 3)()
+    buf = np.zeros(96 * 12 * 512 + 1, np.uint64)
+    lib.drb_phase_timers.restype = C.c_int
+    L.check(lib.drb_phase_timers(C.c_void_p(buf.ctypes.data), dims))
+    ns, nm, nc = dims[0], dims[1], dims[2]
+    assert ns * nm * nc <= buf.size
+    t = buf[:ns * nm * nc].reshape(ns, nm, nc).astype(np.int64)
+    ctas = int((t[0, 0] != 0).sum())
+    steps = min(K, ns)
+    t = t[:steps, :, :ctas]
+    print(json.dumps({"card": card(), "U": U, "I": I, "F": F, "batch": B, "steps": steps, "ctas": ctas}), flush=True)
+    res = {}
+    step_ms = np.median(np.diff(t[:, 0, :].max(axis=1))) / 1e6
+    for name, a, b in SECTIONS:
+        n = steps - 1 if b is None else steps
+        end = t[1:n + 1, 0] if b is None else t[:n, b]
+        per_cta = (end - t[:n, a]).max(axis=1)
+        crit = end.max(axis=1) - t[:n, a].max(axis=1)
+        res[name] = {"max_cta_ms": float(np.median(per_cta)) / 1e6, "critical_ms": float(np.median(crit)) / 1e6}
+    fill = {"norm_fill_ms": float((t[0, 10] - t[0, 9]).max()) / 1e6, "barrier_fill_ms": float((t[0, 11] - t[0, 10]).max()) / 1e6}
+    print(json.dumps({"what": "phase_timers", "step_ms": float(step_ms), "sections": res, "launch": fill}), flush=True)
+    for name, _, _ in SECTIONS:
+        print(f"  {name:16s} max over CTAs {res[name]['max_cta_ms']:.4f} ms   critical path {res[name]['critical_ms']:.4f} ms",
+              flush=True)
 
 
 def timed(fn, steps, reps):
@@ -119,4 +197,9 @@ def main():
 
 
 if __name__ == "__main__":
-    main()
+    if "--timers" in sys.argv:
+        sys.argv.remove("--timers")
+        os.environ["DRB_LIB_PATH"] = timer_lib()
+        phase_timers(int(sys.argv[1]) if len(sys.argv) > 1 else 40)
+    else:
+        main()
